@@ -6,7 +6,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("GS_B200_LIB") or os.path.join(HERE, "libgrayskull_b200.so")   # GS_B200_LIB: A/B variants
+LIB_PATH = os.path.join(HERE, "libgrayskull_b200.so")
 
 
 class Image(C.Structure):  # struct gs_image, reference grayskull.h:14-17

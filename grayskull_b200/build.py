@@ -38,24 +38,18 @@ def _deps_mtime():
     return max(os.path.getmtime(f) for f in files)
 
 
-def build(force=False, verbose=False, defines=(), out=None):
-    """defines/out: experiment variants, e.g. defines=["GSB_BX_BH=32"], out="libvariant.so"
-    (select at run time with GS_B200_LIB=<path>)."""
-    global OBJ
-    lib_out = os.path.join(HERE, out) if out else LIB
-    obj_dir = OBJ if not out else os.path.join(OBJ, os.path.splitext(out)[0])
-    os.makedirs(obj_dir, exist_ok=True)
+def build(force=False, verbose=False):
+    os.makedirs(OBJ, exist_ok=True)
     newest = _deps_mtime()
-    if not force and os.path.exists(lib_out) and os.path.getmtime(lib_out) >= newest:
-        if not out and not os.path.exists(os.path.join(HERE, "gsb_magick")):
+    if not force and os.path.exists(LIB) and os.path.getmtime(LIB) >= newest:
+        if not os.path.exists(os.path.join(HERE, "gsb_magick")):
             build_cli()
-        return lib_out
+        return LIB
     cc = nvcc()
-    dflags = ["-D" + d for d in defines]
 
     def compile_one(src):
-        obj = os.path.join(obj_dir, src.replace(".cu", ".o"))
-        cmd = [cc] + NVCC_FLAGS + dflags + ["-c", os.path.join(CSRC, src), "-o", obj]
+        obj = os.path.join(OBJ, src.replace(".cu", ".o"))
+        cmd = [cc] + NVCC_FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         with open(obj + ".log", "w") as f:
             f.write(r.stdout + r.stderr)
@@ -68,18 +62,15 @@ def build(force=False, verbose=False, defines=(), out=None):
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
     # export only the C ABI (gs_* and the internal gsb_* hooks); C++ symbols stay local
-    vs = os.path.join(obj_dir, "exports.map")
+    vs = os.path.join(OBJ, "exports.map")
     with open(vs, "w") as f:
         f.write("{ global: gs_*; gsb_*; local: *; };\n")
-    cmd = [cc, "-shared", "-o", lib_out] + objs + ["-Xlinker", "--version-script=" + vs]
+    cmd = [cc, "-shared", "-o", LIB] + objs + ["-Xlinker", "--version-script=" + vs]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout + r.stderr)
-    if not out:
-        build_cli()
-    if out:   # experiment variants: their object files are not worth keeping
-        shutil.rmtree(obj_dir, ignore_errors=True)
-    return lib_out
+    build_cli()
+    return LIB
 
 
 def build_cli():
@@ -95,6 +86,4 @@ def build_cli():
 
 
 if __name__ == "__main__":
-    defs = [a.split("=", 1)[1] for a in sys.argv if a.startswith("--define=")]
-    outs = [a.split("=", 1)[1] for a in sys.argv if a.startswith("--out=")]
-    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv, defines=defs, out=outs[0] if outs else None))
+    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

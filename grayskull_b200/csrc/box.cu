@@ -39,26 +39,8 @@ namespace gsb {
 constexpr int BX_STRIDE = 240;             // output columns per tile (lanes 1..30 x 8 pixels)
 constexpr int BX_PW = 64;                  // tile pitch in 32-bit words: image bytes [x0-16, x0+240)
 constexpr int BX_RMAX = 7;
-#ifndef GSB_BX_WARPS
-#define GSB_BX_WARPS 4
-#endif
-#ifndef GSB_BX_BH
-#define GSB_BX_BH 32
-#endif
-#ifndef GSB_BX_HI_XU
-#define GSB_BX_HI_XU 1                     // 1: high-lane float through the conversion pipe (I2F.U16)
-#endif
-#ifndef GSB_BX_LO_XU
-#define GSB_BX_LO_XU 1                     // 1: low lane too
-#endif
-#ifndef GSB_BX_RING
-#define GSB_BX_RING 1
-#endif
-#ifndef GSB_BX_TOT_IMAD
-#define GSB_BX_TOT_IMAD 1                   // 1: lane totals by IMAD x 0x10001 instead of PRMT + add
-#endif
-constexpr int BX_WARPS = GSB_BX_WARPS;     // warps per CTA, one row band each
-constexpr int BX_BH = GSB_BX_BH;           // rows per band
+constexpr int BX_WARPS = 4;                // warps per CTA, one row band each
+constexpr int BX_BH = 32;                  // rows per band
 constexpr int BX_TH = BX_WARPS * BX_BH;    // 128 output rows per tile
 constexpr int BX_THREADS = BX_WARPS * 32;
 constexpr int BX_TILE_WORDS = BX_PW * (BX_TH + 2 * BX_RMAX);
@@ -75,31 +57,18 @@ __host__ __device__ inline DivMagic div_magic(unsigned count) {
   return d;
 }
 
-// floor(s / count) for a 16-bit s, as the low byte of the returned bit pattern
-__device__ __forceinline__ uint32_t div_lo(uint32_t t, float inv, float k) {
-#if GSB_BX_LO_XU
+// floor(s / count) for the low 16-bit lane s of t, as the low byte of the returned bit pattern: float(s) straight
+// from the half on the conversion pipe (I2F.U16, exact), then fma_rd(S, m*2^-24, 2^23) = 2^23 + floor(S*m/2^24)
+__device__ __forceinline__ uint32_t div_lo(uint32_t t, float inv) {
   float fl;
   asm("{ .reg .b16 lo, hi; mov.b32 {lo, hi}, %1; cvt.rn.f32.u16 %0, lo; }" : "=f"(fl) : "r"(t));
-  (void)k;
   return __float_as_uint(__fmaf_rd(fl, inv, 8388608.0f));
-#else
-  return __float_as_uint(__fmaf_rd(__uint_as_float((t & 0xFFFFu) | 0x4B000000u), inv, k));
-#endif
 }
-// high lane: 2^23 + (t >> 16) built with one IMAD.HI (FMA pipe; the ALU pipe is the busy one)
-__device__ __forceinline__ uint32_t div_hi(uint32_t t, float inv, float k) {
-#if GSB_BX_HI_XU
-  // float(t >> 16) straight from the high half on the conversion pipe; exact (16-bit integer), and
-  // fma_rd(S, m*2^-24, 2^23) = 2^23 + floor(S*m/2^24) just like the biased form
+// the same for the high lane
+__device__ __forceinline__ uint32_t div_hi(uint32_t t, float inv) {
   float fh;
   asm("{ .reg .b16 lo, hi; mov.b32 {lo, hi}, %1; cvt.rn.f32.u16 %0, hi; }" : "=f"(fh) : "r"(t));
-  (void)k;
   return __float_as_uint(__fmaf_rd(fh, inv, 8388608.0f));
-#else
-  uint32_t f;
-  asm("mad.hi.u32 %0, %1, 65536, 0x4B000000;" : "=r"(f) : "r"(t));
-  return __float_as_uint(__fmaf_rd(__uint_as_float(f), inv, k));
-#endif
 }
 // low bytes of four 2^23+q floats -> one word; the two 8-bit merges are multiply-adds (FMA pipe)
 __device__ __forceinline__ uint32_t pack4(uint32_t q0, uint32_t q1, uint32_t q2, uint32_t q3) {
@@ -123,8 +92,8 @@ __device__ __forceinline__ void window_sums(const uint32_t (&V)[12], uint32_t (&
 #pragma unroll
   for (int p = 0; p < 4; p++) {
     const int m = M0 + p;
-#if GSB_BX_TOT_IMAD
-    // (ps * 0x10001) >> 16 = lane0 + lane1 (<= 57375, no carry out); * 0x10001 puts it in both lanes
+    // lane totals by IMAD (FMA pipe; the ALU pipe is the busy one): (ps * 0x10001) >> 16 = lane0 + lane1
+    // (<= 57375, no carry out); * 0x10001 puts it in both lanes
     uint32_t x16, tot;
     asm("mad.lo.u32 %0, %1, 0x10001, 0;" : "=r"(x16) : "r"(ps));
     x16 >>= 16;
@@ -136,11 +105,6 @@ __device__ __forceinline__ void window_sums(const uint32_t (&V)[12], uint32_t (&
       asm("mad.lo.u32 %0, %1, 0x10001, 0;" : "=r"(tot) : "r"(x16));
       T[p] = tot - prmt(V[m + R], V[m], 0x5432);
     }
-#else
-    const uint32_t tot = ps + prmt(ps, ps, 0x1032);   // both lanes = lane0 + lane1
-    if (ODD) T[p] = tot + prmt(V[m - 1], V[m + NP], 0x5432);   // + (s_a, s_{a+2R+1})
-    else T[p] = tot - prmt(V[m + R], V[m], 0x5432);            // - (s_{a+2R+1}, s_a)
-#endif
     if (p < 3) ps = ps + V[m + NP] - V[m];
   }
 }
@@ -150,21 +114,19 @@ template <int R, bool INTERIOR>
 __device__ __forceinline__ void box_quot(const uint32_t (&T)[4], const int (&cw)[8], int ch, const float2 *__restrict__ magic,
                                          uint32_t (&q)[8]) {
   constexpr int FULL = 2 * R + 1;
-  constexpr DivMagic FM = {
-      (float)((16777216u + FULL * FULL - 1u) / (FULL * FULL)) * 5.9604644775390625e-08f,
-      8388608.0f - 0.5f * (float)((16777216u + FULL * FULL - 1u) / (FULL * FULL))};
+  constexpr float FINV = (float)((16777216u + FULL * FULL - 1u) / (FULL * FULL)) * 5.9604644775390625e-08f;
   if (INTERIOR) {
 #pragma unroll
     for (int p = 0; p < 4; p++) {
-      q[2 * p] = div_lo(T[p], FM.inv, FM.k);
-      q[2 * p + 1] = div_hi(T[p], FM.inv, FM.k);
+      q[2 * p] = div_lo(T[p], FINV);
+      q[2 * p + 1] = div_hi(T[p], FINV);
     }
   } else {
 #pragma unroll
     for (int p = 0; p < 4; p++) {
       const float2 m0 = magic[cw[2 * p] * ch], m1 = magic[cw[2 * p + 1] * ch];
-      q[2 * p] = div_lo(T[p], m0.x, m0.y);
-      q[2 * p + 1] = div_hi(T[p], m1.x, m1.y);
+      q[2 * p] = div_lo(T[p], m0.x);
+      q[2 * p + 1] = div_hi(T[p], m1.x);
     }
   }
 }
@@ -252,11 +214,9 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
   if (yb >= (int)h) return;                    // warp-uniform
 
   uint32_t S[4] = {0, 0, 0, 0};                // column sums of the 2R rows above the next window row
-#if GSB_BX_RING
   // interior tiles (fully unrolled walk): the unpacked pair words of the 2R+1 rows in the window stay in a register
   // ring, so the row that leaves is not loaded and unpacked a second time (one LDS.64 + four PRMT per row step)
   uint32_t ring[2 * R + 1][4];
-#endif
 #pragma unroll
   for (int i = 0; i < 2 * R; i++) {
     uint32_t e[4];
@@ -264,9 +224,7 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       S[k] += e[k];
-#if GSB_BX_RING
       ring[i][k] = e[k];
-#endif
     }
   }
   uint32_t L[4] = {0, 0, 0, 0};                // the row that leaves the window at this step
@@ -277,16 +235,15 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
     unpack_pairs(*reinterpret_cast<const uint2 *>(in + (i + 2 * R) * BX_PW), e);
 #pragma unroll
     for (int k = 0; k < 4; k++) S[k] = S[k] + e[k] - L[k];   // one IADD3 per word
-#if GSB_BX_RING
     if (INT) {
 #pragma unroll
       for (int k = 0; k < 4; k++) {
         ring[(i + 2 * R) % (2 * R + 1)][k] = e[k];
         L[k] = ring[i % (2 * R + 1)][k];
       }
-    } else
-#endif
-    unpack_pairs(*reinterpret_cast<const uint2 *>(in + i * BX_PW), L);
+    } else {
+      unpack_pairs(*reinterpret_cast<const uint2 *>(in + i * BX_PW), L);
+    }
     // column sums of columns x-8 .. x+15 as pair words V[0..11]; V[4..7] are this lane's own
     uint32_t V[12], T[4];
 #pragma unroll
@@ -332,11 +289,8 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 // blurred rows in registers.  A band of 32 sobel rows needs 34 blurred rows, and sobel needs the blurred columns
 // x-1 / x+8 of the neighbouring lanes, so lanes 2..29 produce outputs: tiles advance 224 columns.  Interior tiles
 // hold neither image column 0 nor w-1, so only the clipped path keeps dst's edge columns.
-#ifndef GSB_BS_UNROLL
-#define GSB_BS_UNROLL 6                       // rows per unrolled step of the interior band loop (0: all 34; the full
+constexpr int BS_UNROLL = 6;                  // rows per unrolled step of the interior band loop (not all 34: the full
                                               // unroll is 74 KB of SASS and stalls on instruction fetch)
-#endif
-constexpr int BS_UNROLL = GSB_BS_UNROLL > 0 ? GSB_BS_UNROLL : BX_BH + 2;
 constexpr int BS_STRIDE = 224;
 constexpr int BS_TILE_WORDS = BX_PW * (BX_TH + 2 + 2 * BX_RMAX);
 constexpr int BS_SMEM = BS_TILE_WORDS * 4 + 226 * 8 + 16;
@@ -637,16 +591,6 @@ k_box_wide(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, int w, in
 //   copy-out: lanes = columns again; rows leave as coalesced 64-bit stores (gs_adaptive_threshold compares
 //             with the centre pixels here, on 16-bit lane pairs).
 // 13.5 lane-instructions per pixel instead of ~37 for k_box_wide (ncu).
-#ifndef GSB_BM_PACK_IMAD
-#define GSB_BM_PACK_IMAD 0                  // 1: byte packing by two IMAD + one PRMT instead of three PRMT (A/B hook)
-#endif
-#ifndef GSB_BM_UNROLL
-#define GSB_BM_UNROLL 1
-#endif
-#ifndef GSB_BM_PF
-#define GSB_BM_PF 0                         // L2 prefetch of the entering rows a chunk ahead: +3 % time saved, +3.6 % instructions: a wash
-#endif
-constexpr int BM_UNROLL = GSB_BM_UNROLL;
 constexpr int BM_PITCH = 130;                       // words per C row
 constexpr int BM_WARP_WORDS = 32 * BM_PITCH + 8;    // + the look-ahead groups of the last row
 constexpr int BM_SMEM = BM_WARP_WORDS * 4;         // one warp per CTA: 16.3 KB, 13 CTAs per SM
@@ -771,7 +715,7 @@ k_box_mid(const __grid_constant__ CUtensorMap tmap, int use_tpf, uint8_t *__rest
   for (int yc = yb; yc < ye; yc += 32) {
     // ---- V-phase: C rows of image rows yc .. yc+31
     __syncwarp();                                               // the previous chunk's copy-out is done
-    pf_box(yc + r + 13 + 32 * use_tpf);                         // what the next chunk's ring loads will ask for (use_tpf: chunks ahead)
+    pf_box(yc + r + 13 + 32 * use_tpf);                         // what the next chunk's ring loads will ask for
     auto v_phase = [&](auto guard_tag) {
       uint32_t *crow = cs + 2 + 4 * lane;
 #pragma unroll 1
@@ -781,13 +725,6 @@ k_box_mid(const __grid_constant__ CUtensorMap tmap, int use_tpf, uint8_t *__rest
           const int yn = yc + 16 * bb + 4 * qb + 12;            // first row step of the batch three ahead
           ld_batch(en[(qb + 3) & 3], yn + r + 1, guard_tag);
           ld_batch(lv[(qb + 3) & 3], yn - r, guard_tag);
-#if GSB_BM_PF
-          if (!decltype(guard_tag)::value) {                    // L2 prefetch of the entering rows one chunk further down
-            const uint8_t *pp = col + (size_t)(unsigned)(yn + r + 1) * wl;
-#pragma unroll
-            for (int k = 0; k < 4; k++) asm volatile("prefetch.global.L2 [%0];" ::"l"(pp + (size_t)(k + 32) * wl));
-          }
-#endif
 #pragma unroll
           for (int k = 0; k < 4; k++) {
             *reinterpret_cast<uint2 *>(crow) = make_uint2(S[0], S[1]);
@@ -881,11 +818,7 @@ k_box_mid(const __grid_constant__ CUtensorMap tmap, int use_tpf, uint8_t *__rest
               q[k] = q0 & 0xFFu;
             }
           }
-#if GSB_BM_PACK_IMAD
-          ow[s] = pack4(q[0], q[1], q[2], q[3]);
-#else
           ow[s] = pack4_alu(q[0], q[1], q[2], q[3]);
-#endif
         }
         asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(po_s + 8 * t), "r"(ow[0]), "r"(ow[1]) : "memory");
       };
@@ -911,7 +844,7 @@ k_box_mid(const __grid_constant__ CUtensorMap tmap, int use_tpf, uint8_t *__rest
 #pragma unroll 1
         for (; t < t_end; t++) single(t, std::false_type{});
         if (seg == 0) {
-#pragma unroll BM_UNROLL
+#pragma unroll 1
           for (; t + 1 < t_hi && t + 1 <= u_in; t += 2) {       // A -> B -> A: no register rotation; look-ahead inside the row
             step8(t, std::true_type{}, std::false_type{}, EA, LA, EB[1], LB[1], EB, LB);
             step8(t + 1, std::true_type{}, std::false_type{}, EB, LB, EA[1], LA[1], EA, LA);
@@ -1060,8 +993,7 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
     const int fast_ok = (r <= 63 && box_wide_magic((2 * r + 1) * (2 * r + 1), &minv)) ? 1 : 0;
     const bool aligned = w % 8 == 0 && reinterpret_cast<uintptr_t>(src) % 8 == 0 && reinterpret_cast<uintptr_t>(dst) % 8 == 0;
     dim3 grid((strips + 3) / 4, gy, n);
-    static const bool use_mid = [] { const char *e = getenv("GS_B200_BOX"); return !(e && e[0] == 'w'); }();   // A/B hook: "wide"
-    if (aligned && use_mid) {
+    if (aligned) {
       // k_box_mid: chunks of 32 rows, so bands are multiples of 32 rows.  Short bands keep the grid many waves deep
       // (3 CTAs of 4 warps per SM); a band re-reads 2r + 1 + 12 rows of its upper neighbour (L2 hits) and spends ~7
       // instructions on each, against ~75 per regular row: the largest of 128 / 64 / 32 rows that still gives
@@ -1071,14 +1003,11 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
       for (int cand = 128; cand >= 32; cand >>= 1)
         if ((long long)strips * ((h + cand - 1) / cand) * n >= four_waves || cand == 32) { BH = cand; break; }
       while (BH < 4 * (int)r && BH < 256) BH <<= 1;
-      static const int bh_env = [] { const char *e = getenv("GS_B200_BOX_BH"); return e ? atoi(e) : 0; }();   // A/B hook
-      if (bh_env >= 32) BH = bh_env / 32 * 32;
       const long long warps = (long long)strips * ((h + BH - 1) / BH);
       GSB_ASSERT(warps < (1ll << 31));
       grid = dim3((unsigned)warps, 1, n);
       CUtensorMap pmap;
-      static const int tpf_env = [] { const char *e = getenv("GS_B200_BOX_TPF"); return e ? atoi(e) : 1; }();   // A/B hook: 0 = off, k = k chunks ahead
-      int use_tpf = (tpf_env > 0 && make_tmap_u8frames(&pmap, src, w, h, n, 72, 32)) ? tpf_env : 0;   // needs w % 16 == 0 and a 16-byte aligned base
+      const int use_tpf = make_tmap_u8frames(&pmap, src, w, h, n, 72, 32) ? 1 : 0;   // needs w % 16 == 0 and a 16-byte aligned base
       if (!use_tpf) memset(&pmap, 0, sizeof(pmap));
       static DeviceOnce once;
       if (once.needed()) {

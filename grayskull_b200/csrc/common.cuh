@@ -122,14 +122,9 @@ __device__ __forceinline__ uint32_t prmt_raw(uint32_t a, uint32_t b, uint32_t se
   asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(sel));
   return d;
 }
-// streaming 64/128-bit stores (outputs are written once and not re-read by the same kernel)
+// streaming 64-bit store (outputs are written once and not re-read by the same kernel)
 __device__ __forceinline__ void st_cs_u2(void *p, uint2 v) {
   asm volatile("st.global.cs.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(v.x), "r"(v.y) : "memory");
-}
-__device__ __forceinline__ void st_cs_u4(void *p, uint4 v) {
-  asm volatile("st.global.cs.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z),
-               "r"(v.w)
-               : "memory");
 }
 #endif  // __CUDACC__
 

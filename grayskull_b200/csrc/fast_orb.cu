@@ -1,17 +1,17 @@
 // fast_orb.cu -- gs_fast, gs_compute_orientation, gs_brief_descriptor, gs_orb_extract
 // (reference grayskull.h:482-669).
 //
-// gs_fast      pass 1  k_fast_score : FAST-9 score map, interior pixels only.  16-bit brighter /
-//                                     darker ring masks; "run of >= 9" is the rotate-AND test; the
-//                                     unsigned-wrap quirk of reference :498 (p < t => every
-//                                     non-brighter sample counts as darker) is reproduced.
-//              (k_fast_score_tiled is the batched form: smem tile, compass pre-test, candidate
-//              compaction; k_fast_score the per-pixel form for foreign-sized score maps)
-//              pass 2  k_nms_mask -> k_row_scan -> k_nms_emit_masks : 3x3 strict-greater NMS over the
-//                                     caller's score map (including the ring cells pass 1 never
-//                                     writes, exactly like reference :517-524) and a SCAN-based
-//                                     compaction, because the reference emits keypoints in raster
-//                                     order and stops at nkps (:530).
+// gs_fast      pass 1  k_fast_tiled2 : FAST-9 score map, interior pixels only, and the 3x3 strict-greater
+//                                     NMS bits of each row (smem tile, compass pre-test, candidate
+//                                     compaction).  16-bit brighter / darker ring masks; "run of >= 9"
+//                                     is the rotate-AND test; the unsigned-wrap quirk of reference :498
+//                                     (p < t => every non-brighter sample counts as darker) is reproduced.
+//                                     Foreign-sized score maps, force_generic and thresholds above 255
+//                                     take the per-pixel k_fast_score and then k_nms_mask instead.
+//              pass 2  k_row_scan -> k_nms_emit_masks : the NMS over the caller's score map (including
+//                                     the ring cells pass 1 never writes, exactly like reference
+//                                     :517-524) ends in a SCAN-based compaction, because the reference
+//                                     emits keypoints in raster order and stops at nkps (:530).
 // gs_orb_extract       k_orb_select : one CTA per frame: stable descending counting sort on the
 //                                     8-bit response (== the reference's bubble sort, :639-649),
 //                                     15-px margin filter and cap, all order-preserving.
@@ -236,16 +236,15 @@ struct KpRec {  // struct gs_keypoint, 48 bytes
 };
 
 // ---------------------------------------------------------------------------------------------
-// Tiled FAST score (used when the score map has the image's size): a CTA owns a 128 x 16 pixel
-// tile.  The source tile (+3 halo) is staged in shared memory; every pixel runs the cheap compass
-// pre-test (any 9-arc contains two of the ring positions 0/4/8/12); the few candidates are
-// compacted into a dense list so that the full 16-sample test runs with full warps (in v1 one
-// candidate lane dragged its whole warp through it); scores are assembled in shared memory and
-// written out row-wise.  Arc test on sign bits: funnel-shifting the sign of (hi - v) / (v - lo)
-// into the masks costs one IADD and one SHF per sample and mask.
-// ---------------------------------------------------------------------------------------------
-constexpr int FT_W = 128, FT_H = 16, FT_SW = FT_W + 32, FT_SH = FT_H + 6;   // 160-B pitch = one TMA box row
-constexpr int FT_X = 16;                                                   // tile byte of the first pixel column
+// Tiled FAST (used when the score map has the image's size and t <= 255): a CTA stages its source tile (+3 halo)
+// in shared memory; every pixel runs a cheap compass pre-test on 16-bit lane pairs, 4 pixels per thread: with
+// K = 0x7FFF - t per lane, bit 15 of (v + K - p) is "v > p + t" and bit 15 of (p + K - v) is "v < p - t"; bit 15
+// of (0x7FFF + t - p) is the wrap case t > p (reference :498), where every non-brighter sample counts as darker.
+// The few candidates are compacted into a dense list so that the full 16-sample test runs with full warps (with
+// one thread per pixel, one candidate lane dragged its whole warp through it).  Arc test on sign bits:
+// funnel-shifting the sign of (hi - v) / (v - lo) into the masks costs one IADD and one SHF per sample and mask.
+constexpr int FT_W = 128, FT_SW = FT_W + 32;   // tile columns; 160-B pitch = one TMA box row
+constexpr int FT_X = 16;                        // tile byte of the first pixel column
 
 // 4 bytes -> 16-bit lane pairs (b0, b2) and (b1, b3)
 __device__ __forceinline__ void pairs_eo(uint32_t v, uint32_t &e, uint32_t &o) {
@@ -253,166 +252,10 @@ __device__ __forceinline__ void pairs_eo(uint32_t v, uint32_t &e, uint32_t &o) {
   o = prmt(v, 0, 0x4341);
 }
 
-template <bool TMA>
-__global__ void __launch_bounds__(256)
-k_fast_score_tiled(const __grid_constant__ CUtensorMap tmap, const uint8_t *__restrict__ src, unsigned w, unsigned h,
-                   uint8_t *__restrict__ score, unsigned t) {
-  __shared__ __align__(128) uint8_t s_src[FT_SH * FT_SW];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ __align__(16) uint8_t s_score[FT_H * FT_W];
-  __shared__ uint16_t s_list[FT_H * FT_W];
-  __shared__ unsigned s_cnt;
-  const unsigned f = blockIdx.z, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  // tile = pixel columns [x0, x0+128) (x0 a multiple of 128: aligned words), interior rows [y0, y0+16)
-  const int x0 = blockIdx.x * FT_W, y0 = 3 + blockIdx.y * FT_H;
-  const uint8_t *img = src + (size_t)f * w * h;
-  if (tid == 0) s_cnt = 0;
-  // stage rows y0-3 .. y0+18, columns x0-16 .. x0+143
-  if (TMA) {
-    if (tid == 0) {
-      mbar_init(&bar, 1);
-      mbar_fence_init();
-    }
-    __syncthreads();
-    if (tid == 0) {
-      mbar_expect_tx(&bar, FT_SH * FT_SW);
-      tma_load_3d(s_src, &tmap, (x0 - FT_X) / 4, y0 - 3, (int)f, &bar);   // out-of-image reads as 0, never used
-    }
-  } else {
-    for (int i = tid; i < FT_SH * FT_SW; i += 256) {
-      const int r = i / FT_SW, c = i % FT_SW;
-      const int yy = min(y0 - 3 + r, (int)h - 1), xx = min(max(x0 - FT_X + c, 0), (int)w - 1);
-      s_src[i] = __ldg(img + (size_t)yy * w + xx);
-    }
-  }
-  for (int i = tid; i < FT_H * FT_W / 4; i += 256) reinterpret_cast<uint32_t *>(s_score)[i] = 0;
-  if (TMA) mbar_wait(&bar, 0);
-  __syncthreads();
-
-  // phase A: compass pre-test (any 9-arc contains two of ring positions 0/4/8/12), 4 pixels per
-  // thread on 16-bit lane pairs.  With K = 0x7FFF - t per lane, bit 15 of (v + K - p) is "v > p + t"
-  // and bit 15 of (p + K - v) is "v < p - t"; bit 15 of (0x7FFF + t - p) is the wrap case t > p
-  // (reference :498), where every non-brighter sample counts as darker.  "at least two of four"
-  // = (a&b) | (c&d) | ((a|b) & (c|d)), "at least three" = (a&b&(c|d)) | (c&d&(a|b)), bitwise.
-  {
-    const int lx = 4 * lane;                                // first of this thread's 4 pixel columns
-    const unsigned tc = min(t, 0x7000u);                    // thresholds above 255 all behave alike
-    const uint32_t kb = (0x7FFFu - tc) * 0x10001u, kw = (0x7FFFu + tc) * 0x10001u;
-    unsigned colmask = 0;                                   // interior columns: 3 <= x < w - 3
-#pragma unroll
-    for (int j = 0; j < 4; j++) colmask |= (unsigned)(x0 + lx + j >= 3 && x0 + lx + j + 3 < (int)w) << j;
-    unsigned flags = 0;                                     // bit 4k + j: row warp + 8k, pixel j is a candidate
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-      const int ly = warp + 8 * k;
-      const uint32_t *rowc = reinterpret_cast<const uint32_t *>(s_src + (ly + 3) * FT_SW) + (FT_X / 4) + lane;
-      const uint32_t wl = rowc[-1], wc = rowc[0], wr = rowc[1];
-      const uint32_t up = rowc[-3 * (FT_SW / 4)], dn = rowc[3 * (FT_SW / 4)];
-      const uint32_t v12 = __funnelshift_r(wl, wc, 8);      // bytes x-3 .. x
-      const uint32_t v4 = __funnelshift_r(wc, wr, 24);      // bytes x+3 .. x+6
-      uint32_t pe, po, ve[4], vo[4];
-      pairs_eo(wc, pe, po);
-      pairs_eo(up, ve[0], vo[0]);
-      pairs_eo(v4, ve[1], vo[1]);
-      pairs_eo(dn, ve[2], vo[2]);
-      pairs_eo(v12, ve[3], vo[3]);
-      unsigned cbits = 0;
-#pragma unroll
-      for (int hlf = 0; hlf < 2; hlf++) {
-        const uint32_t P = hlf ? po : pe;
-        const uint32_t q = kb - P, r = P + kb, wrap = kw - P;
-        uint32_t b[4], d[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          const uint32_t V = hlf ? vo[i] : ve[i];
-          b[i] = V + q;
-          d[i] = r - V;
-        }
-        const uint32_t two_b = (b[0] & b[1]) | (b[2] & b[3]) | ((b[0] | b[1]) & (b[2] | b[3]));
-        const uint32_t two_d = (d[0] & d[1]) | (d[2] & d[3]) | ((d[0] | d[1]) & (d[2] | d[3]));
-        const uint32_t three_b = (b[0] & b[1] & (b[2] | b[3])) | (b[2] & b[3] & (b[0] | b[1]));
-        const uint32_t cand = two_b | (wrap & ~three_b) | (~wrap & two_d);
-        // lanes: hlf 0 -> pixels 0 and 2, hlf 1 -> pixels 1 and 3
-        cbits |= ((cand >> 15) & 1u) << hlf;
-        cbits |= (cand >> 31) << (2 + hlf);
-      }
-      if (y0 + ly + 3 < (int)h) flags |= (cbits & colmask) << (4 * k);
-    }
-    // one compaction per thread: warp-exclusive scan of the per-thread candidate counts, one
-    // shared-memory atomic per warp (candidates are rare: the common case is an all-zero ballot)
-    if (__any_sync(0xFFFFFFFFu, flags != 0)) {
-      const unsigned c = __popc(flags);
-      unsigned incl = c;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const unsigned u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-        if (lane >= (unsigned)o) incl += u;
-      }
-      unsigned base = 0;
-      if (lane == 31) base = atomicAdd(&s_cnt, incl);
-      base = __shfl_sync(0xFFFFFFFFu, base, 31) + incl - c;
-      while (flags) {
-        const int bit = __ffs(flags) - 1;
-        flags &= flags - 1;
-        s_list[base++] = (uint16_t)((warp + 8 * (bit >> 2)) * FT_W + lx + (bit & 3));
-      }
-    }
-  }
-  __syncthreads();
-
-  // phase B: full test on the dense candidate list
-  const unsigned ncand = s_cnt;
-  for (unsigned k = tid; k < ncand; k += 256) {
-    const int i = s_list[k], ly = i / FT_W, lx = i % FT_W;
-    const uint8_t *c = s_src + (ly + 3) * FT_SW + (lx + FT_X);
-    const int p = c[0], hi = p + (int)t, lo = p - (int)t;
-    unsigned bright = 0, dark = 0;
-    int mind = 255;
-#define FAST_TAP2(i_, dx, dy)                                                       \
-  {                                                                                 \
-    const int v = c[(dy) * FT_SW + (dx)];                                           \
-    bright = __funnelshift_l((unsigned)(hi - v), bright, 1);   /* bit = (v > hi) */  \
-    dark = __funnelshift_l((unsigned)(v - lo), dark, 1);       /* bit = (v < lo) */  \
-    mind = min(mind, abs(v - p));                                                   \
-  }
-    FAST_RING(FAST_TAP2)
-#undef FAST_TAP2
-    bright &= 0xFFFFu;
-    // reference :498: when t > p the unsigned p - t wraps and every non-brighter sample is "darker"
-    dark = (t > (unsigned)p) ? (~bright & 0xFFFFu) : (dark & 0xFFFFu);
-    // the masks are bit-reversed w.r.t. the ring index (sample 0 ends up in bit 15): circular
-    // runs are invariant under reversal
-    if (run9(bright) || run9(dark)) s_score[i] = (uint8_t)mind;
-  }
-  __syncthreads();
-
-  // phase C: write the tile's scores, interior pixels only (3 <= x < w-3): a word per 4 pixels
-  {
-    const int lx = 4 * lane;
-    unsigned colmask = 0;
-#pragma unroll
-    for (int j = 0; j < 4; j++) colmask |= (unsigned)(x0 + lx + j >= 3 && x0 + lx + j + 3 < (int)w) << j;
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-      const int ly = warp + 8 * k, y = y0 + ly;
-      if (y + 3 >= (int)h || colmask == 0) continue;
-      const uint32_t v = *reinterpret_cast<const uint32_t *>(s_score + ly * FT_W + lx);
-      uint8_t *q = score + (size_t)f * w * h + (size_t)y * w + x0 + lx;
-      if (colmask == 0xF && TMA) {            // (TMA <=> w % 16 == 0 and aligned bases: word stores are aligned)
-        *reinterpret_cast<uint32_t *>(q) = v;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-          if ((colmask >> j) & 1u) q[j] = (uint8_t)(v >> (8 * j));
-      }
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // k_fast_tiled2: FAST score AND the 3x3 non-maximum mask of a tile in one kernel (round 2).
 // Round 1 ran k_nms_mask as a second, latency-bound pass over the score map (1.1 TB/s) that the score kernel
-// had just held in shared memory.  Here a CTA scores an 18-row x 130-column region -- its 16 x 128 tile plus a
+// had just held in shared memory.  Here a CTA scores a 66-row x 130-column region -- its 64 x 128 tile plus a
 // 1-pixel ring, recomputed instead of exchanged -- and derives the tile's NMS bits straight from shared memory.
 // Ring cells that FAST never writes (x = 2, x = w-3, y = 2, y = h-3: whatever the caller left in the map takes
 // part in the NMS, reference :517-524) are fetched from the global score map; nobody writes those, so there is
@@ -1101,8 +944,7 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
   GSB_ASSERT(n <= 65535u && rows <= 0x7FFFFFFFu);
   // thresholds above 255 (the reference computes p + t / p - t in unsigned arithmetic, :496-498, which wraps for
   // huge t) take the literal per-pixel kernel: the tiled kernel's 16-bit lane arithmetic assumes t <= 255
-  const char *unf = getenv("GS_B200_FAST_UNFUSED");     // A/B hook: 1 = round 1's two kernels (score, then NMS mask)
-  if (sw == w && sh == h && !force_generic() && threshold <= 255u && !(unf && unf[0] && unf[0] != '0')) {
+  if (sw == w && sh == h && !force_generic() && threshold <= 255u) {
     // score + NMS mask in one kernel (k_fast_tiled2); the per-row counts are accumulated with atomics
     dim3 grid((w + FT_W - 1) / FT_W, (h - 6 + F2_TH - 1) / F2_TH, n);
     GSB_ASSERT(grid.y <= 65535u);
@@ -1116,20 +958,10 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
     }
     GSB_LAUNCHED(1);
   } else {
-    if (sw == w && sh == h && !force_generic() && threshold <= 255u) {
-      dim3 grid((w + FT_W - 1) / FT_W, (h - 6 + FT_H - 1) / FT_H, n);
-      GSB_ASSERT(grid.y <= 65535u);
-      CUtensorMap tmap;
-      if (tma_ok(src, w) && tma_ok(score, w) && make_tmap_u8frames(&tmap, src, w, h, n, FT_SW / 4, FT_SH))
-        k_fast_score_tiled<true><<<grid, 256, 0, s>>>(tmap, src, w, h, score, threshold);
-      else {
-        memset(&tmap, 0, sizeof(tmap));
-        k_fast_score_tiled<false><<<grid, 256, 0, s>>>(tmap, src, w, h, score, threshold);
-      }
-    } else {   // foreign-sized score map (single-image gs_fast only): gs_set semantics per pixel
-      dim3 block(32, 8), grid((w - 6 + 31) / 32, (h - 6 + 7) / 8, n);
-      k_fast_score<<<grid, block, 0, s>>>(src, w, h, n, score, sw, sh, threshold);
-    }
+    // foreign-sized score map (single-image gs_fast only), force_generic or t > 255: gs_set semantics per pixel,
+    // then the NMS mask as a second pass
+    dim3 block(32, 8), grid((w - 6 + 31) / 32, (h - 6 + 7) / 8, n);
+    k_fast_score<<<grid, block, 0, s>>>(src, w, h, n, score, sw, sh, threshold);
     GSB_LAUNCHED(1);
     if (sw % 4 == 0 && reinterpret_cast<uintptr_t>(score) % 4 == 0 && sw >= w && sh >= h)   // word pre-test stays inside the map
       k_nms_mask<true><<<dim3((rows + 7) / 8, n), 256, 0, s>>>(score, sw, sh, w, h, mw, masks, rowcount);

@@ -202,13 +202,7 @@ k_integral_bands(uint32_t *__restrict__ ii, const uint8_t *__restrict__ src, uns
 // (byte masks 0x01, 0x0101, ...) accumulated straight onto previous row + offset.  ~4.5 instructions per pixel
 // instead of 13.5, ~50-100 registers.  The next RB rows are requested before the current ones are scanned.  Tickets
 // are handed out strip-major, so a strip's left neighbours always hold earlier tickets (resident or done).
-#ifndef GSB_IS_MINB
-#define GSB_IS_MINB 4
-#endif
-#ifndef GSB_IS_CS
-#define GSB_IS_CS 0
-#endif
-constexpr int IS_MINB = GSB_IS_MINB;         // CTAs of 128 threads per SM the register allocation must allow
+constexpr int IS_MINB = 4;                   // CTAs of 128 threads per SM the register allocation must allow
 
 template <int IS_TPB, int RB>
 __global__ void __launch_bounds__(IS_TPB, IS_MINB * 128 / IS_TPB)
@@ -298,14 +292,9 @@ k_integral_strips(uint32_t *__restrict__ ii, const uint8_t *__restrict__ src, un
           prev[5] = __dp4a(px[r].y, 0x00000101u, prev[5] + base2);
           prev[6] = __dp4a(px[r].y, 0x00010101u, prev[6] + base2);
           prev[7] = __dp4a(px[r].y, ONES, prev[7] + base2);
-#if GSB_IS_CS
-          st_cs_u4(q, make_uint4(prev[0], prev[1], prev[2], prev[3]));       // streaming: the table is not re-read here
-          st_cs_u4(q + 4, make_uint4(prev[4], prev[5], prev[6], prev[7]));
-#else
           uint4 *q4 = reinterpret_cast<uint4 *>(q);
           q4[0] = make_uint4(prev[0], prev[1], prev[2], prev[3]);
           q4[1] = make_uint4(prev[4], prev[5], prev[6], prev[7]);
-#endif
           q += w;
         }
       }
@@ -330,7 +319,7 @@ extern "C" int gs_b200_integral_batch(uint32_t *ii, const uint8_t *src, unsigned
     const unsigned sw_cols = narrow ? 512u : 1024u, rb = narrow ? 16u : 8u;
     const unsigned strips = (w + sw_cols - 1) / sw_cols, nbands = (h + rb - 1) / rb;
     const unsigned long long ctas = (unsigned long long)n * strips;
-    const char *env = getenv("GS_B200_INTEGRAL");      // test / A-B hook: "bands" or "strips"
+    const char *env = getenv("GS_B200_INTEGRAL");      // test hook: "bands" or "strips"
     const bool want = env ? env[0] == 's' : ctas >= sms;
     if (want && !(env && env[0] == 'b') && w % 8 == 0 && strips <= 16 && aligned && !gsb::force_generic() && ctas < 0x7FFFFFFFull) {
       const size_t slot_bytes = sizeof(unsigned long long) * (size_t)ctas * nbands * rb;

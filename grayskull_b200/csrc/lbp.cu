@@ -16,9 +16,11 @@
 //             shared memory (warp ballot + one atomic per warp), so later stages run with full
 //             warps instead of a few live lanes (v1 measured 7.8 of 32 lanes active).  Stage sums
 //             are accumulated with sequential fp32 adds exactly as :808.  Hits are recorded as one
-//             bit per window, which keeps the reference's order for free;
-//   k_lbp_scan3  : the default for step-2 scans of 8-px-aligned tables (GS_B200_LBP_TMA=0 selects
-//             k_lbp_scan2): the same cascade walk on a 2-D window tile whose integral-image boxes (even- and
+//             bit per window, which keeps the reference's order for free.  It takes the scans
+//             k_lbp_scan3 cannot: step != 2, iw % 8 != 0, a table base that is not 16-byte aligned,
+//             force_generic, or a scale whose tile does not fit;
+//   k_lbp_scan3  : step-2 scans of 8-px-aligned, 16-byte-aligned tables whose features stay inside
+//             their window: the same cascade walk on a 2-D window tile whose integral-image boxes (even- and
 //             odd-column planes made by k_deinterleave2, so that step-2 windows gather from adjacent words)
 //             are staged into shared memory by two TMA bulk-tensor copies (zero fill = the x == 0 / y == 0
 //             corner rule); each warp re-packs its own survivors (no CTA barriers) and finishes its last few
@@ -49,15 +51,9 @@ struct FeatGeo {               // corner lattice of one feature at one scale, as
   int row[4];                  // (fy - 1 + j*fh) * iw
   int col[4];                  // fx - 1 + i*fw
 };
-#ifndef GSB_LBP_SLOTS
-#define GSB_LBP_SLOTS 128
-#endif
-#ifndef GSB_LBP_THREADS
-#define GSB_LBP_THREADS 256
-#endif
-constexpr int LBP_SLOTS_PER_CTA = GSB_LBP_SLOTS;            // 32 windows each
+constexpr int LBP_SLOTS_PER_CTA = 128;                      // 32 windows each
 constexpr int LBP_WIN_PER_CTA = LBP_SLOTS_PER_CTA * 32;
-constexpr int LBP_THREADS = GSB_LBP_THREADS;
+constexpr int LBP_THREADS = 256;
 constexpr int LBP_MAX_GROUPS = 8;
 struct Weak {
   float left, right;
@@ -178,25 +174,10 @@ k_lbp_scan(const uint32_t *__restrict__ ii_all, unsigned iw, unsigned ih, DevCas
 }
 
 // the 8-bit LBP code from the eight neighbour cells (clockwise from top-left, reference :776-782) and the centre
-#ifndef GSB_LBP_FSHIFT
-#define GSB_LBP_FSHIFT 0
-#endif
-
 __device__ __forceinline__ int lbp_code_of(uint32_t n7, uint32_t n6, uint32_t n5, uint32_t n4, uint32_t n3, uint32_t n2,
                                            uint32_t n1, uint32_t n0, uint32_t m) {
-#if GSB_LBP_FSHIFT
-  // EXPERIMENT (not measured yet, off by default): cell sums are far below 2^31, so `cell >= centre` is the
-  // inverted sign of cell - centre; a funnel shift appends that sign to the code word: 2 instructions per bit
-  // instead of compare + select + or.
-  uint32_t acc = 0;
-  acc = __funnelshift_l(n7 - m, acc, 1), acc = __funnelshift_l(n6 - m, acc, 1), acc = __funnelshift_l(n5 - m, acc, 1);
-  acc = __funnelshift_l(n4 - m, acc, 1), acc = __funnelshift_l(n3 - m, acc, 1), acc = __funnelshift_l(n2 - m, acc, 1);
-  acc = __funnelshift_l(n1 - m, acc, 1), acc = __funnelshift_l(n0 - m, acc, 1);
-  return (int)(~acc & 0xFFu);
-#else
   return ((n7 >= m) << 7) | ((n6 >= m) << 6) | ((n5 >= m) << 5) | ((n4 >= m) << 4) | ((n3 >= m) << 3) | ((n2 >= m) << 2) |
          ((n1 >= m) << 1) | ((n0 >= m) << 0);
-#endif
 }
 
 // one weak classifier for one window (reference gs_lbp_code + gs_lbp_match, :769-788)
@@ -379,21 +360,10 @@ k_deinterleave2(uint32_t *__restrict__ planes, const uint32_t *__restrict__ ii, 
   }
 }
 
-#ifndef GSB_LBP3_THREADS
-#define GSB_LBP3_THREADS 512
-#endif
-#ifndef GSB_LBP_ROWDIFF
-#define GSB_LBP_ROWDIFF 1
-#endif
-#ifndef GSB_LBP3_GRAB
-#define GSB_LBP3_GRAB 0
-#endif
-#ifndef GSB_LBP3_FLAT
-#define GSB_LBP3_FLAT 8        // a warp with this many survivors or fewer switches to the (window, weak) flat mode
-#endif
-constexpr int LBP3_THREADS = GSB_LBP3_THREADS;   // small-window scales: two CTAs per SM
+constexpr int LBP3_THREADS = 512;                // small-window scales: two CTAs per SM
 constexpr int LBP3_BIG_THREADS = 1024;           // large-window scales: one CTA per SM with a tile up to 224 KB
 constexpr int LBP3_HIT_WORDS = 128;              // mask words of a tile: at most 4096 windows
+constexpr int LBP3_FLAT = 8;                     // flat_n: a warp with this many survivors or fewer switches to the (window, weak) flat mode
 
 template <int LBP3_THREADS>
 __global__ void __launch_bounds__(LBP3_THREADS)
@@ -461,10 +431,8 @@ k_lbp_scan3(const __grid_constant__ CUtensorMap tmap, DevCascade dc, int si, int
 #pragma unroll
       for (int k = 0; k < 4; k++) v[j][k] = *reinterpret_cast<const uint32_t *>(rb + g.col[k]);
     }
-    uint32_t c[3][3];
-#if GSB_LBP_ROWDIFF
     // cell = D + A - B - C as a difference of horizontal differences: 12 + 9 subtractions instead of 27 add/subs
-    uint32_t hd[4][3];
+    uint32_t c[3][3], hd[4][3];
 #pragma unroll
     for (int j = 0; j < 4; j++)
 #pragma unroll
@@ -473,12 +441,6 @@ k_lbp_scan3(const __grid_constant__ CUtensorMap tmap, DevCascade dc, int si, int
     for (int j = 0; j < 3; j++)
 #pragma unroll
       for (int k = 0; k < 3; k++) c[j][k] = hd[j + 1][k] - hd[j][k];
-#else
-#pragma unroll
-    for (int j = 0; j < 3; j++)
-#pragma unroll
-      for (int k = 0; k < 3; k++) c[j][k] = v[j + 1][k + 1] + v[j][k] - v[j][k + 1] - v[j + 1][k];
-#endif
     const uint32_t m = c[1][1];
     const int code = lbp_code_of(c[0][0], c[0][1], c[0][2], c[1][2], c[2][2], c[2][1], c[2][0], c[1][0], m);
     const int idx = code >> 5;
@@ -500,6 +462,9 @@ k_lbp_scan3(const __grid_constant__ CUtensorMap tmap, DevCascade dc, int si, int
   // warp + nwarps, ... (static; a warp whose slots hold the faces of the tile finishes long after the others, and the CTA
   // keeps its tile and warp slots until then: 24 of 32 warp slots occupied on average, ncu); grab > 0: `grab`
   // consecutive slots at a time from a shared counter, taken through all stage groups before the next hand-out.
+  // The launcher always passes grab = 0.  The hand-out still stays in the kernel: without it, nvcc 12.9 compiles
+  // the static walk to code that ran c4 1.2 % slower (570.1 vs 563.3 ms per step, median of three alternated runs,
+  // H100 80GB HBM3 at 400 W), also with the grab parameter kept and take fixed at 0.
   constexpr int NWARPS = LBP3_THREADS / 32;
   const unsigned warp = tid >> 5, lt = (1u << lane) - 1u;
   const int nslots = nwin >> 5;
@@ -672,19 +637,12 @@ struct PlanKey {
   unsigned iw, ih;
   float sf, mn, mx;
   int step, device;
-  int tuning;                  // the tile-planning environment hooks (tests / A-B runs flip them inside one process)
+  int big_mode;                // GS_B200_LBP_BIG (a test flips it inside one process): -1 auto, 0 never, 1 always
   bool operator==(const PlanKey &o) const {
     return hash == o.hash && iw == o.iw && ih == o.ih && sf == o.sf && mn == o.mn && mx == o.mx && step == o.step &&
-           device == o.device && tuning == o.tuning;
+           device == o.device && big_mode == o.big_mode;
   }
 };
-static int plan_tuning() {
-  auto geti = [](const char *name, int dflt) {
-    const char *e = getenv(name);
-    return e ? atoi(e) : dflt;
-  };
-  return geti("GS_B200_LBP_TILE_KB", 113) * 65536 + (geti("GS_B200_LBP_BIG", -1) + 2) * 4096 + geti("GS_B200_LBP_BIG_ROWS", 32);
-}
 struct PlanEntry {
   PlanKey key;
   void *blob = nullptr;
@@ -764,7 +722,10 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
                         int step) {
   int dev = 0;
   cudaGetDevice(&dev);
-  PlanKey key = {cascade_hash(c), iw, ih, sf, mn, mx, step, dev, plan_tuning()};
+  // test hook: 1 = every scale on the 1024-thread tile form, 0 = none, unset = by tile height (tests reach both
+  // forms on frames where the automatic choice takes only one)
+  const char *be = getenv("GS_B200_LBP_BIG");
+  PlanKey key = {cascade_hash(c), iw, ih, sf, mn, mx, step, dev, be ? atoi(be) : -1};
   std::lock_guard<std::mutex> lock(g_plan_mutex);
   for (auto &r : g_plans)
     if (r->key == key) return r;
@@ -804,10 +765,8 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
   // per-CTA shared-memory budget (tile planes + tables + survivor lists): 113 KB lets two 512-thread CTAs share an
   // SM at every scale (round 1 bounded the planes alone by 100 KB, and scale 10 of the UHD ladder came out at
   // 119.9 KB: one CTA per SM, 705 us instead of ~500)
-  size_t tile_budget = (size_t)113 * 1024;
-  if (const char *tb = getenv("GS_B200_LBP_TILE_KB")) tile_budget = (size_t)atoi(tb) * 1024;
-  int big_auto_rows = 32;                                            // scales whose 2-per-SM tile has fewer window rows go big
-  if (const char *br = getenv("GS_B200_LBP_BIG_ROWS")) big_auto_rows = atoi(br);
+  const size_t tile_budget = (size_t)113 * 1024;
+  const int big_auto_rows = 32;                                      // scales whose 2-per-SM tile has fewer window rows go big
   std::vector<TileGeo> tgeo;
   bool tiles_ok = safe && ns > 0 && iw % 8 == 0 && step == 2;
   for (int s2 = 0; s2 < ns && tiles_ok; s2++) {
@@ -846,9 +805,7 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
     TilePlan small, big;
     fit(LBP3_THREADS, tile_budget, 2048, small);
     fit(LBP3_BIG_THREADS, (size_t)224 * 1024, 32 * LBP3_HIT_WORDS, big);
-    int big_mode = -1;                                             // -1 auto, 0 never, 1 always (A/B hook)
-    if (const char *be = getenv("GS_B200_LBP_BIG")) big_mode = atoi(be);
-    const bool use_big = big.twy > 0 && (big_mode == 1 || (big_mode < 0 && small.twy < big_auto_rows));
+    const bool use_big = big.twy > 0 && (key.big_mode == 1 || (key.big_mode < 0 && small.twy < big_auto_rows));
     tp = use_big ? big : small;
     if (!tp.twy) {
       tiles_ok = false;
@@ -907,16 +864,7 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
   e.dc.tgeo = reinterpret_cast<const TileGeo *>(b + o_tg);
   e.dc.nweaks = nw, e.dc.nsubsets = (int)nsub;
   {  // stage groups: re-pack after each of the first stages (most windows die there), then coarser
-    int cuts[7] = {1, 2, 3, 4, 6, 9, 13};
-    if (const char *ce = getenv("GS_B200_LBP_CUTS")) {      // tuning hook: up to 7 ascending stage indices, "1,2,3,5"
-      int k = 0;
-      for (const char *q = ce; *q && k < 7;) {
-        cuts[k++] = atoi(q);
-        while (*q && *q != ',') q++;
-        if (*q == ',') q++;
-      }
-      for (; k < 7; k++) cuts[k] = 1 << 20;
-    }
+    const int cuts[7] = {1, 2, 3, 4, 6, 9, 13};
     int ng = 0;
     for (int k = 0; k < 7 && ng < LBP_MAX_GROUPS - 1; k++)
       if (cuts[k] < nst) e.dc.group_end[ng++] = cuts[k];
@@ -977,10 +925,7 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
   const size_t smem2 = table_bytes + 2 * sizeof(uint16_t) * gsb::LBP_WIN_PER_CTA;
   // k_lbp_scan3 (TMA-staged parity-plane tiles, warp-autonomous survivor lists) when the scan is the usual
   // step-2 one on 8-px-aligned tables; bit-exact with k_lbp_scan2, half its instructions.
-  // GS_B200_LBP_TMA=0 selects k_lbp_scan2.
-  const char *tma_env = getenv("GS_B200_LBP_TMA");
-  const bool v3 = !p->tiles.empty() && reinterpret_cast<uintptr_t>(ii) % 16 == 0 && !gsb::force_generic() &&
-                  !(tma_env && tma_env[0] == '0') && getenv("GS_B200_LBP_V1") == nullptr;
+  const bool v3 = !p->tiles.empty() && reinterpret_cast<uintptr_t>(ii) % 16 == 0 && !gsb::force_generic();
   if (v3) {
     static gsb::DeviceOnce once3;
     if (once3.needed()) {
@@ -989,10 +934,6 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
       once3.done();
     }
     GSB_CHECK(cudaMemsetAsync(masks, 0, 4 * (size_t)dc.total_slots * n, st));   // padding slots between scales
-    int flat_n = GSB_LBP3_FLAT;
-    if (const char *fe = getenv("GS_B200_LBP_FLAT")) flat_n = atoi(fe);
-    int grab = GSB_LBP3_GRAB;                 // slots per dynamic hand-out, 0 = static slot assignment
-    if (const char *ge = getenv("GS_B200_LBP_GRAB")) grab = atoi(ge);
     // frames go through in chunks so that the de-interleaved copy stays small (<= 1 GiB of workspace)
     const size_t frame_bytes = (size_t)iw * ih * 4;
     unsigned chunk = (unsigned)(((size_t)1 << 30) / frame_bytes);
@@ -1013,10 +954,10 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
           return gsb::record_error(cudaErrorInvalidValue, __FILE__, __LINE__);
         if (tp.threads == gsb::LBP3_BIG_THREADS)
           gsb::k_lbp_scan3<gsb::LBP3_BIG_THREADS><<<dim3((unsigned)(tp.tiles_x * tp.tiles_y), nf), gsb::LBP3_BIG_THREADS, tp.smem, st>>>(
-              tm, dc, si, tp.twx, tp.twy, tp.bw, tp.ph, tp.tiles_x, flat_n, grab, masks + (size_t)f0 * dc.total_slots);
+              tm, dc, si, tp.twx, tp.twy, tp.bw, tp.ph, tp.tiles_x, gsb::LBP3_FLAT, 0, masks + (size_t)f0 * dc.total_slots);
         else
           gsb::k_lbp_scan3<gsb::LBP3_THREADS><<<dim3((unsigned)(tp.tiles_x * tp.tiles_y), nf), gsb::LBP3_THREADS, tp.smem, st>>>(
-              tm, dc, si, tp.twx, tp.twy, tp.bw, tp.ph, tp.tiles_x, flat_n, grab, masks + (size_t)f0 * dc.total_slots);
+              tm, dc, si, tp.twx, tp.twy, tp.bw, tp.ph, tp.tiles_x, gsb::LBP3_FLAT, 0, masks + (size_t)f0 * dc.total_slots);
         GSB_LAUNCHED(1);
       }
     }
@@ -1028,8 +969,7 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
     GSB_LAUNCHED(1);
     return 0;
   }
-  const bool v2 = dc.safe_geometry && smem2 <= 160 * 1024 && (unsigned long long)iw * ih < 0x7FFFFFFFull &&
-                  getenv("GS_B200_LBP_V1") == nullptr;
+  const bool v2 = dc.safe_geometry && smem2 <= 160 * 1024 && (unsigned long long)iw * ih < 0x7FFFFFFFull;
   if (v2) {
     static gsb::DeviceOnce once2;
     if (once2.needed()) {                         // the v2 condition above caps smem2 at 160 KB

@@ -22,13 +22,10 @@ struct MatchRec {
 };
 constexpr int MT_CHUNK = 256;   // candidate descriptors per shared-memory chunk
 
-#ifndef GSB_MATCH_CSA
-#define GSB_MATCH_CSA 2
-#endif
 // popcount of 8 words.  POPC issues at 16 lanes/clk/SM against 64 for LOP3, so 8 POPCs per comparison
-// bound the plain form.  A carry-save adder tree (LOP3 pairs:
-// 0x96 sum, 0xE8 majority) compresses the words first; GSB_MATCH_CSA picks how far: 1 -> 6 POPC + 4 LOP3,
-// 2 -> 5 POPC + 6 LOP3 (balances the two pipes), 3 -> 4 POPC + 14 LOP3 (ALU-bound again).
+// bound the plain form.  A carry-save adder tree (LOP3 pairs: 0x96 sum, 0xE8 majority) compresses the
+// words first.  Two levels (5 POPC + 6 LOP3) balance the two pipes: one level (6 POPC + 4 LOP3) leaves
+// POPC the bound, three (4 POPC + 14 LOP3) make the ALU pipe the bound again.
 __device__ __forceinline__ void csa(uint32_t a, uint32_t b, uint32_t c, uint32_t &sum, uint32_t &carry) {
   // explicit LOP3s (0x96 = a^b^c, 0xE8 = majority): left to itself nvcc folds the caller's q^d xors into
   // 4-input expressions and spends ~50 % more LOP3s
@@ -36,30 +33,11 @@ __device__ __forceinline__ void csa(uint32_t a, uint32_t b, uint32_t c, uint32_t
   asm("lop3.b32 %0, %1, %2, %3, 0xE8;" : "=r"(carry) : "r"(a), "r"(b), "r"(c));
 }
 __device__ __forceinline__ unsigned popc8(const uint32_t (&x)[8]) {
-#if GSB_MATCH_CSA == 3
-  uint32_t s1, c1, s2, c2, s3, c3, t1, d1;
-  csa(x[0], x[1], x[2], s1, c1);
-  csa(x[3], x[4], x[5], s2, c2);
-  csa(s1, s2, x[6], s3, c3);
-  const uint32_t ones = s3 ^ x[7], c4 = s3 & x[7];
-  csa(c1, c2, c3, t1, d1);
-  const uint32_t twos = t1 ^ c4, d2 = t1 & c4;
-  const uint32_t fours = d1 ^ d2, eights = d1 & d2;
-  return __popc(ones) + 2 * __popc(twos) + 4 * __popc(fours) + 8 * __popc(eights);
-#elif GSB_MATCH_CSA == 2
   uint32_t s1, c1, s2, c2, s3, c3;
   csa(x[0], x[1], x[2], s1, c1);
   csa(x[3], x[4], x[5], s2, c2);
   csa(s1, s2, x[6], s3, c3);
   return __popc(s3) + __popc(x[7]) + 2 * (__popc(c1) + __popc(c2) + __popc(c3));
-#elif GSB_MATCH_CSA == 1
-  uint32_t s1, c1, s2, c2;
-  csa(x[0], x[1], x[2], s1, c1);
-  csa(x[3], x[4], x[5], s2, c2);
-  return __popc(s1) + __popc(s2) + __popc(x[6]) + __popc(x[7]) + 2 * (__popc(c1) + __popc(c2));
-#else
-  return __popc(x[0]) + __popc(x[1]) + __popc(x[2]) + __popc(x[3]) + __popc(x[4]) + __popc(x[5]) + __popc(x[6]) + __popc(x[7]);
-#endif
 }
 
 // Scan state in the integer domain: key = distance << 22 | candidate index, so that min() over keys also
@@ -68,10 +46,7 @@ __device__ __forceinline__ unsigned popc8(const uint32_t (&x)[8]) {
 // d < M <=> d < thr, so a key replaces the M stand-in exactly when the reference's fp32 compare does,
 // and a state still >= thr << 22 at the end means "M".
 constexpr int MT_IDX_BITS = 22;
-#ifndef GSB_MATCH_QPW
-#define GSB_MATCH_QPW 2          // queries per warp: each staged candidate is read once for QPW queries
-#endif
-constexpr int MT_QPW = GSB_MATCH_QPW;
+constexpr int MT_QPW = 2;            // queries per warp: each staged candidate is read once for QPW queries
 constexpr int MT_QPC = 8 * MT_QPW;   // queries per CTA
 
 __global__ void __launch_bounds__(256)

@@ -60,10 +60,6 @@ __device__ __forceinline__ void resize_axis(unsigned i, unsigned sdim, unsigned 
 // ONE 64-bit load instead of eight byte gathers, and the u8 -> f32 conversions pick their byte straight out
 // of the loaded words.  Threads that do not qualify (other ratios, clamped edges) take the gather path.
 constexpr int RS_ROWS = 8;
-#ifndef GSB_RS_PAIRS
-#define GSB_RS_PAIRS 1
-#endif
-
 
 __device__ __forceinline__ float bilerp(float c00, float c01, float c10, float c11, float omx, float dx, float omy,
                                         float dy) {
@@ -74,29 +70,17 @@ __device__ __forceinline__ float bilerp(float c00, float c01, float c10, float c
   return p;
 }
 // u8 -> f32 and f32 -> u8 without the conversion pipe (I2F / F2I run at 16 lanes/clk/SM and four conversions per
-// dst pixel capped round 1's kernel at ~4 pixels/clk/SM): 0x4B0000bb is the float 2^23 + bb, so one PRMT (ALU pipe)
-// and one exact FADD (FMA pipe) give float(bb); adding 2^23 to p in [0, 256) with round-toward-zero leaves
+// dst pixel capped round 1's kernel at ~4 pixels/clk/SM): adding 2^23 to p in [0, 256) with round-toward-zero leaves
 // trunc(p) in the low byte.
 //
-// [r2] GSB_RS_DENORM: the u8 -> f32 step disappears altogether.  The bit pattern of a byte b read as a float IS the
+// [r2] The u8 -> f32 step needs no arithmetic.  The bit pattern of a byte b read as a float IS the
 // subnormal b * 2^-149, and a power-of-two scaling commutes with round-to-nearest as long as nothing leaves the normal
 // range: rn(b * 2^-149 * (wx * 2^126)) = rn(b * wx) * 2^-23 and rn(that * (wy * 2^23)) = rn(rn(b * wx) * wy), the
 // reference's two products bit for bit (b * wx >= 2^-11 or 0; the weights are pre-scaled once per thread / per row;
 // FMUL takes subnormal inputs at full rate, the library is built without -ftz).  Per tap: load + 2 FMUL.
-#ifndef GSB_RS_DENORM
-#define GSB_RS_DENORM 1
-#endif
-#if GSB_RS_DENORM
 constexpr float RS_WX_SCALE = 0x1p126f, RS_WY_SCALE = 0x1p23f;
 __device__ __forceinline__ float byte_f(uint32_t w, int k) { return __uint_as_float(prmt(w, 0u, 0x4440u | (unsigned)k)); }
 __device__ __forceinline__ float u8_f(unsigned b) { return __uint_as_float(b); }
-#else
-constexpr float RS_WX_SCALE = 1.0f, RS_WY_SCALE = 1.0f;
-__device__ __forceinline__ float byte_f(uint32_t w, int k) {
-  return __fsub_rn(__uint_as_float(prmt(w, 0x4B000000u, 0x7540u | (unsigned)k)), 8388608.0f);
-}
-__device__ __forceinline__ float u8_f(unsigned b) { return __fsub_rn(__uint_as_float(b | 0x4B000000u), 8388608.0f); }
-#endif
 __device__ __forceinline__ uint32_t f_trunc_bits(float p) { return __float_as_uint(__fadd_rz(p, 8388608.0f)); }  // low byte = (uint8_t)p
 
 template <bool VEC>
@@ -127,7 +111,7 @@ k_resize(uint8_t *__restrict__ dst, unsigned dw, unsigned dh, const uint8_t *__r
     omx[j] = __fmul_rn(__fsub_rn(1.0f, dx[j]), RS_WX_SCALE);
     dx[j] = __fmul_rn(dx[j], RS_WX_SCALE);
   }
-  bool pairs = GSB_RS_PAIRS && VEC && src_aligned8 && x0[0] % 8 == 0 && x + 3 < dw;
+  bool pairs = VEC && src_aligned8 && x0[0] % 8 == 0 && x + 3 < dw;
 #pragma unroll
   for (int j = 0; j < 4; j++) pairs = pairs && x0[j] == x0[0] + 2 * j && x1[j] == x0[j] + 1;
   for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
@@ -299,10 +283,9 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
     const unsigned cols = (unsigned)(127.0 * rx) + 22, rows = (unsigned)((8.0 * gsb::RS_ROWS - 1) * ry) + 6;   // spare: fp32 vs double, 16-byte alignment
     const unsigned pitch = (cols + 15) / 16 * 16;
     const size_t bytes = (size_t)pitch * rows;
-    const char *env = getenv("GS_B200_RESIZE");          // A/B hook: "gather" forces the round-1 kernel
     const bool pairs_case = aligned8 && sw == 2 * dw;     // exact 2:1 in x: the 64-bit pair loads of k_resize are already good
     CUtensorMap tm;
-    if (bytes <= (size_t)gsb::RT_MAX_BYTES && pitch <= 1024 && rows <= 256 && !(env && env[0] == 'g') && !pairs_case &&
+    if (bytes <= (size_t)gsb::RT_MAX_BYTES && pitch <= 1024 && rows <= 256 && !pairs_case &&
         gsb::tma_ok(src, sw) && n <= 65535u && gsb::make_tmap_u8frames(&tm, src, sw, sh, n, pitch / 4, rows)) {
       static gsb::DeviceOnce once;
       if (once.needed()) {
