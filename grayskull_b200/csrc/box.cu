@@ -287,13 +287,41 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 // packing and storing them, the lane fetches its neighbours' edge quotients by two shuffles and builds gs_sobel's
 // pair words with one PRMT each (pairs.cuh: quot_pairs), keeping the horizontal partials of the previous two
 // blurred rows in registers.  A band of 32 sobel rows needs 34 blurred rows, and sobel needs the blurred columns
-// x-1 / x+8 of the neighbouring lanes, so lanes 2..29 produce outputs: tiles advance 224 columns.  Interior tiles
-// hold neither image column 0 nor w-1, so only the clipped path keeps dst's edge columns.
+// x-1 / x+8 of the neighbouring lanes, so lanes 2..29 produce outputs: tiles advance 224 columns.
+// The path is chosen per warp and per lane, not per tile: a warp whose 34 blurred rows all have unclipped row
+// windows takes the unrolled loop, whatever the other warps of its tile do; only the frame's top and bottom bands
+// (and partial bands) take the clipped loop, which reads the division table.  Column clipping never leaves the
+// unrolled loop: each lane divides by its own eight counts (a constant unless it holds column 0 or w-1).  The lanes
+// holding column 0 or w-1 keep dst's byte there by writing the other seven bytes as three stores, so the kernel
+// never reads dst.
 constexpr int BS_UNROLL = 6;                  // rows per unrolled step of the interior band loop (not all 34: the full
                                               // unroll is 74 KB of SASS and stalls on instruction fetch)
 constexpr int BS_STRIDE = 224;
 constexpr int BS_TILE_WORDS = BX_PW * (BX_TH + 2 + 2 * BX_RMAX);
 constexpr int BS_SMEM = BS_TILE_WORDS * 4 + 226 * 8 + 16;
+
+// division of one row of 8 pixels by the lane's own per-pixel reciprocals inv[i] (see div_magic)
+__device__ __forceinline__ void box_quot_lanes(const uint32_t (&T)[4], const float (&inv)[8], uint32_t (&q)[8]) {
+#pragma unroll
+  for (int p = 0; p < 4; p++) {
+    q[2 * p] = div_lo(T[p], inv[2 * p]);
+    q[2 * p + 1] = div_hi(T[p], inv[2 * p + 1]);
+  }
+}
+
+// the 8 output bytes of a lane whose first byte is image column 0 (left) or whose last is column w-1 (!left): the
+// other seven bytes as three aligned stores, so that dst's border byte stays as it was without being read
+__device__ __forceinline__ void st_cs_7of8(uint8_t *p, uint2 v, bool left) {
+  if (left) {
+    asm volatile("st.global.cs.u8 [%0], %1;" ::"l"(p + 1), "r"(v.x >> 8) : "memory");
+    asm volatile("st.global.cs.u16 [%0], %1;" ::"l"(p + 2), "r"(v.x >> 16) : "memory");
+    asm volatile("st.global.cs.u32 [%0], %1;" ::"l"(p + 4), "r"(v.y) : "memory");
+  } else {
+    asm volatile("st.global.cs.u32 [%0], %1;" ::"l"(p), "r"(v.x) : "memory");
+    asm volatile("st.global.cs.u16 [%0], %1;" ::"l"(p + 4), "r"(v.y) : "memory");
+    asm volatile("st.global.cs.u8 [%0], %1;" ::"l"(p + 6), "r"(v.y >> 16) : "memory");
+  }
+}
 
 template <int R>
 __global__ void __launch_bounds__(BX_THREADS)
@@ -308,38 +336,48 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
   const unsigned frame = blockIdx.z;
   const int xb = (int)blockIdx.x * BS_STRIDE - 16;   // image column of tile byte 0 (16-B aligned)
   const int y0 = (int)blockIdx.y * BX_TH;            // first sobel row of the tile
-  // every window of the blurred pixels this tile needs (rows y0-1 .. y0+TH, columns xb+8 .. xb+247) is unclipped
-  const bool interior = xb + 8 - R >= 0 && xb + 8 + BX_STRIDE - 1 + R <= (int)w - 1 && y0 - 1 - R >= 0 &&
-                        y0 + BX_TH + R <= (int)h - 1;
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
     mbar_fence_init();
+    mbar_expect_tx(&bar, BX_PW * 4 * ROWS);
+    tma_load_3d(tile, &tmap, xb / 4, y0 - 1 - R, frame, &bar);
   }
-  if (!interior) {
+  // the clipped-count division table, only where some warp's band has row-clipped windows (the tile holds the
+  // frame's first or last rows); it is built while the tile is in flight
+  if (y0 - 1 - R < 0 || y0 + BX_TH + R > (int)h - 1) {
     for (unsigned c = threadIdx.x + 1; c < 226; c += BX_THREADS) {
       const DivMagic d = div_magic(c);
       magic[c] = make_float2(d.inv, d.k);
     }
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(&bar, BX_PW * 4 * ROWS);
-    tma_load_3d(tile, &tmap, xb / 4, y0 - 1 - R, frame, &bar);
-  }
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int x = xb + 8 * lane;
   const int yb = y0 + warp * BX_BH;            // first sobel row of this warp's band; blurred rows yb-1 .. yb+BH
+  // every row window of the band's blurred rows is unclipped: the unrolled loop.  Warp-uniform; the vote tells the
+  // compiler so, and the loop's shuffles then need no convergence check
+  const bool rows_full = __all_sync(0xFFFFFFFFu, yb - 1 - R >= 0 && yb + BX_BH + R <= (int)h - 1);
   const bool blur_lane = lane >= 1 && lane <= 30 && x >= 0 && x < (int)w;
   const bool out_lane = lane >= 2 && lane <= 29 && x < (int)w;
   const uint32_t *in = tile + (warp * BX_BH) * BX_PW + 2 * lane;   // tile row of image row yb - 1 - R
   uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
-  // the quotients of lanes outside the image are wrong (count 1) and may exceed 255: an output lane takes only the
-  // low byte of its neighbours' edge quotients (quot_pairs), which then feeds only pixel x (left neighbour outside:
-  // x = 0) or x+7 (right neighbour outside: x+7 = w-1), and both keep dst's bytes
+  // the quotients of lanes outside the image are wrong (made-up counts) and may exceed 255: an output lane takes
+  // only the low byte of its neighbours' edge quotients (quot_pairs), which then feeds only pixel x (left neighbour
+  // outside: x = 0) or x+7 (right neighbour outside: x+7 = w-1), and both keep dst's bytes
   int cw[8];
 #pragma unroll
   for (int j = 0; j < 8; j++) cw[j] = blur_lane ? min(x + j + R, (int)w - 1) - max(x + j - R, 0) + 1 : 1;
+  // the unrolled loop's per-pixel reciprocals of count = cw * (2R+1): the same values as the table's, a constant
+  // except in the lanes of columns 0 and w-8 (R <= 7 < 8), the only ones with clipped column windows
+  constexpr float FINV = (float)((16777216u + FULL * FULL - 1u) / (FULL * FULL)) * 5.9604644775390625e-08f;
+  float inv[8];
+#pragma unroll
+  for (int j = 0; j < 8; j++) inv[j] = FINV;
+  if (blur_lane && (x - R < 0 || x + 7 + R > (int)w - 1)) {
+#pragma unroll
+    for (int j = 0; j < 8; j++) inv[j] = div_magic(cw[j] * FULL).inv;
+  }
   const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
 
   mbar_wait(&bar, 0);
@@ -371,28 +409,35 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
       V[8 + k] = (R == 7 || k < 3) ? __shfl_down_sync(0xFFFFFFFFu, S[k], 1) : 0u;
     }
     window_sums<R>(V, T);
-    int ch = FULL;
-    if (!INT) {
+    if (INT) {
+      box_quot_lanes(T, inv, q);
+    } else {
       const int y = yb - 1 + j;
-      ch = max(min(y + R, (int)h - 1) - max(y - R, 0) + 1, 1);   // rows outside the image are never used
+      const int ch = max(min(y + R, (int)h - 1) - max(y - R, 0) + 1, 1);   // rows outside the image are never used
+      box_quot<R, false>(T, cw, ch, magic, q);
     }
-    box_quot<R, INT>(T, cw, ch, magic, q);
   };
 
+  // the lanes of columns 0 and w-1 keep dst's byte there; all three stores are predicated, no lane branches
+  const bool st_all = out_lane && !edge_l && !edge_r, st_l = out_lane && edge_l, st_r = out_lane && edge_r;
+  const bool edge_warp = __any_sync(0xFFFFFFFFu, st_l || st_r);
+  auto store = [&](uint2 so) {
+    if (st_all) st_cs_u2(outp, so);
+    if (st_l) st_cs_7of8(outp, so, true);
+    if (st_r) st_cs_7of8(outp, so, false);
+  };
   SobelRow ra, rb;
-  auto sobel_step = [&](int j, const uint32_t (&q)[8], bool write_row, auto interior_tag) {
+  auto sobel_step = [&](int j, const uint32_t (&q)[8], bool write_row, auto interior_tag, auto edge_tag) {
     const uint32_t qm1 = __shfl_up_sync(0xFFFFFFFFu, q[7], 1);    // blurred pixel x-1
     const uint32_t q8 = __shfl_down_sync(0xFFFFFFFFu, q[0], 1);   // blurred pixel x+8
     const SobelRow rc = sobel_row(quot_pairs(qm1, q, q8));
     if (j >= 2) {
       if (decltype(interior_tag)::value) {
         const uint2 so = sobel_out(ra, rb, rc);  // outside the branch, so that the store is predicated
-        if (out_lane) st_cs_u2(outp, so);
-      } else if (write_row && out_lane) {
-        uint2 so = sobel_out(ra, rb, rc);
-        if (edge_l) so.x = (so.x & 0xFFFFFF00u) | outp[0];                        // keep dst(0, y)
-        if (edge_r) so.y = (so.y & 0x00FFFFFFu) | ((uint32_t)outp[7] << 24);      // keep dst(w-1, y)
-        st_cs_u2(outp, so);
+        if (decltype(edge_tag)::value) store(so);
+        else if (out_lane) st_cs_u2(outp, so);
+      } else if (write_row) {
+        store(sobel_out(ra, rb, rc));
       }
       outp += w;
     }
@@ -400,13 +445,18 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
     rb = rc;
   };
 
-  if (interior) {
+  // unrolled walk; a warp with a lane on column 0 or w-1 gets its own copy, so that the others store as before
+  auto walk_rows_full = [&](auto edge_tag) {
 #pragma unroll BS_UNROLL
     for (int j = 0; j < BX_BH + 2; j++) {
       uint32_t q[8];
       blur_row(j, std::true_type{}, q);
-      sobel_step(j, q, true, std::true_type{});
+      sobel_step(j, q, true, std::true_type{}, edge_tag);
     }
+  };
+  if (rows_full) {
+    if (edge_warp) walk_rows_full(std::true_type{});
+    else walk_rows_full(std::false_type{});
   } else {
 #pragma unroll 1
     for (int j = 0; j < BX_BH + 2; j++) {
@@ -414,7 +464,7 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
       if (ys > (int)h - 2) break;                // warp-uniform
       uint32_t q[8];
       blur_row(j, std::false_type{}, q);
-      sobel_step(j, q, ys >= 1, std::false_type{});
+      sobel_step(j, q, ys >= 1, std::false_type{}, std::true_type{});
     }
   }
 }
