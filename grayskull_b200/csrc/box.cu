@@ -287,7 +287,10 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 // packing and storing them, the lane fetches its neighbours' edge quotients by two shuffles and builds gs_sobel's
 // pair words with one PRMT each (pairs.cuh: quot_pairs), keeping the horizontal partials of the previous two
 // blurred rows in registers.  A band of 32 sobel rows needs 34 blurred rows, and sobel needs the blurred columns
-// x-1 / x+8 of the neighbouring lanes, so lanes 2..29 produce outputs: tiles advance 224 columns.
+// x-1 / x+8 of the neighbouring lanes.  Lanes 0 and 31 hand on one blurred pixel each, lane 0 its pixel 7 and lane
+// 31 its pixel 0: window_sums<R> gets those two right for every R <= 7, because their windows use only V[4..11]
+// and V[0..7] (lane 0's V[0..3] enter the rolling sum and leave it again exactly, mod 2^32).  So lanes 1..30
+// produce outputs and tiles advance 240 columns, as in k_box_tma.
 // The path is chosen per warp and per lane, not per tile: a warp whose 34 blurred rows all have unclipped row
 // windows takes the unrolled loop, whatever the other warps of its tile do; only the frame's top and bottom bands
 // (and partial bands) take the clipped loop, which reads the division table.  Column clipping never leaves the
@@ -296,7 +299,7 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 // never reads dst.
 constexpr int BS_UNROLL = 6;                  // rows per unrolled step of the interior band loop (not all 34: the full
                                               // unroll is 74 KB of SASS and stalls on instruction fetch)
-constexpr int BS_STRIDE = 224;
+constexpr int BS_STRIDE = 240;                // output columns per tile (lanes 1..30 x 8 pixels)
 constexpr int BS_TILE_WORDS = BX_PW * (BX_TH + 2 + 2 * BX_RMAX);
 constexpr int BS_SMEM = BS_TILE_WORDS * 4 + 226 * 8 + 16;
 
@@ -358,8 +361,10 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
   // every row window of the band's blurred rows is unclipped: the unrolled loop.  Warp-uniform; the vote tells the
   // compiler so, and the loop's shuffles then need no convergence check
   const bool rows_full = __all_sync(0xFFFFFFFFu, yb - 1 - R >= 0 && yb + BX_BH + R <= (int)h - 1);
-  const bool blur_lane = lane >= 1 && lane <= 30 && x >= 0 && x < (int)w;
-  const bool out_lane = lane >= 2 && lane <= 29 && x < (int)w;
+  // lanes 0 and 31 need the right counts for the pixel they hand on; the first tile's lane 1 sits at column -8, so
+  // its outputs start at lane 2
+  const bool blur_lane = x >= 0 && x < (int)w;
+  const bool out_lane = lane >= 1 && lane <= 30 && x >= 0 && x < (int)w;
   const uint32_t *in = tile + (warp * BX_BH) * BX_PW + 2 * lane;   // tile row of image row yb - 1 - R
   uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
   // the quotients of lanes outside the image are wrong (made-up counts) and may exceed 255: an output lane takes
@@ -1093,7 +1098,7 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
 
 template <int R>
 static int launch_blur_sobel_r(const CUtensorMap &tmap, uint8_t *dst, unsigned w, unsigned h, unsigned n, cudaStream_t s) {
-  const unsigned tiles_x = (w + BS_STRIDE - 1) / BS_STRIDE, tiles_y = (h + BX_TH - 1) / BX_TH;
+  const unsigned tiles_x = (w + 8 + BS_STRIDE - 1) / BS_STRIDE, tiles_y = (h + BX_TH - 1) / BX_TH;
   GSB_ASSERT(tiles_y <= 65535u && n <= 65535u);
   static DeviceOnce once;
   if (once.needed()) {
