@@ -100,6 +100,8 @@ SIGNATURES = {
     "gs_b200_blur_sobel_batch": (_i, [_p, _p, _u, _u, _u, _u, _p]),
     "gs_b200_erode_batch": (_i, [_p, _p, _u, _u, _u, _p]),
     "gs_b200_dilate_batch": (_i, [_p, _p, _u, _u, _u, _p]),
+    "gs_b200_erode_n_batch": (_i, [_p, _p, _u, _u, _u, _u, _p]),
+    "gs_b200_dilate_n_batch": (_i, [_p, _p, _u, _u, _u, _u, _p]),
     "gs_b200_resize_batch": (_i, [_p, _u, _u, _p, _u, _u, _u, _p]),
     "gs_b200_downsample_batch": (_i, [_p, _p, _u, _u, _u, _p]),
     "gs_b200_integral_batch": (_i, [_p, _p, _u, _u, _u, _p]),

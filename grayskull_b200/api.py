@@ -220,6 +220,28 @@ def dilate_batch(src, out=None):
     return out
 
 
+def erode_n_batch(src, iters, out=None):
+    """`iters` passes of the 3x3 erode in one call (bit-identical to `iters` chained erode_batch calls)"""
+    import torch
+    n, h, w = _chk_frames(src)
+    if not 0 <= iters < 2 ** 32:
+        raise ValueError("iters must be in [0, 2**32), got %r" % (iters,))
+    out = torch.empty_like(src) if out is None else out
+    check(lib().gs_b200_erode_n_batch(_p(out), _p(src), w, h, n, iters, _stream()), "erode_n_batch")
+    return out
+
+
+def dilate_n_batch(src, iters, out=None):
+    """`iters` passes of the 3x3 dilate in one call (bit-identical to `iters` chained dilate_batch calls)"""
+    import torch
+    n, h, w = _chk_frames(src)
+    if not 0 <= iters < 2 ** 32:
+        raise ValueError("iters must be in [0, 2**32), got %r" % (iters,))
+    out = torch.empty_like(src) if out is None else out
+    check(lib().gs_b200_dilate_n_batch(_p(out), _p(src), w, h, n, iters, _stream()), "dilate_n_batch")
+    return out
+
+
 def resize_batch(src, dw, dh, out=None):
     import torch
     n, h, w = _chk_frames(src)

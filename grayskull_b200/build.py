@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libgrayskull_b200.so")
 SOURCES = ["runtime.cu", "stencil3.cu", "box.cu", "resample.cu", "integral.cu", "fast_orb.cu", "match.cu", "histogram.cu", "filter.cu", "lbp.cu", "blobs.cu",
-           "api.cu"]
+           "morph.cu", "api.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-fmad=false", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
               "-I", os.path.join(os.path.dirname(HERE), "include")]

@@ -8,6 +8,7 @@
  * taken through the pipeline without leaving the device (two ping-pong frame batches), copied back once
  * and written as <out-prefix>NNNN.pgm.  Pipeline = comma-separated stages, arguments after ':'
  *   blur:R   sobel   erode[:N]   dilate[:N]   adaptive:R:C   threshold:T   threshold:otsu[+K]
+ *   (erode:N / dilate:N are N passes of the 3x3 op in one call, gs_b200_erode_n_batch / gs_b200_dilate_n_batch)
  *   filter:sharpen|emboss|box|gaussian   downsample   resize:W:H
  *   keypoints:N:T   (prints the ORB keypoint count per frame; frames pass through unchanged)
  *   blobs:N         (prints the number of 4-connected components >= 128 per frame; frames pass through unchanged)
@@ -60,14 +61,11 @@ static void stage(const char *spec, struct batch *cur, struct batch *tmp, size_t
     CK(gs_b200_memset(tmp->dev, 0, frame_bytes(cur) * n, NULL)); /* gs_alloc'ed dst: zero frame */
     CK(gs_b200_sobel_batch(tmp->dev, cur->dev, w, h, n, NULL));
   } else if ((!strcmp(name, "erode") || !strcmp(name, "dilate")) && nargs <= 1) {
-    int reps = nargs == 1 ? atoi(a0) : 1, i;
+    int reps = nargs == 1 ? atoi(a0) : 1;
     if (reps <= 0) DIE("bad repeat count in '%s'", spec);
     ensure(tmp, w, h, n, cap_tmp);
-    for (i = 0; i < reps; i++) {
-      if (name[0] == 'e') CK(gs_b200_erode_batch(tmp->dev, cur->dev, w, h, n, NULL));
-      else CK(gs_b200_dilate_batch(tmp->dev, cur->dev, w, h, n, NULL));
-      if (i + 1 < reps) t = *cur, *cur = *tmp, *tmp = t, tc = *cap_cur, *cap_cur = *cap_tmp, *cap_tmp = tc;
-    }
+    if (name[0] == 'e') CK(gs_b200_erode_n_batch(tmp->dev, cur->dev, w, h, n, (unsigned)reps, NULL));
+    else CK(gs_b200_dilate_n_batch(tmp->dev, cur->dev, w, h, n, (unsigned)reps, NULL));
   } else if (!strcmp(name, "adaptive") && nargs == 2) {
     ensure(tmp, w, h, n, cap_tmp);
     CK(gs_b200_adaptive_threshold_batch(tmp->dev, cur->dev, w, h, n, (unsigned)atoi(a0), atoi(a1), NULL));

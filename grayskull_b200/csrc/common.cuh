@@ -58,7 +58,7 @@ struct DeviceOnce {
   void done() { mask.fetch_or(bit(), std::memory_order_release); }
 };
 enum { WS_INTEGRAL = 0, WS_FAST_A, WS_FAST_B, WS_ORB_A, WS_ORB_B, WS_LBP_A, WS_LBP_B, WS_LBP_C,
-       WS_STAGE_A, WS_STAGE_B, WS_STAGE_C, WS_STAGE_D, WS_HIST, WS_STAGE_FUSED, WS_BLOB_A, WS_BLOB_B, WS_BLOB_C, WS_SLOTS };
+       WS_STAGE_A, WS_STAGE_B, WS_STAGE_C, WS_STAGE_D, WS_HIST, WS_STAGE_FUSED, WS_BLOB_A, WS_BLOB_B, WS_BLOB_C, WS_MORPH, WS_SLOTS };
 
 // 3-D tensor map over n dense u8 frames of w x h, viewed as 32-bit words {w/4, h, n}
 // (TMA boxes are limited to 256 elements per dimension: u32 elements give 1 KiB wide boxes).

@@ -74,6 +74,17 @@ int gs_b200_erode_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h
                         gs_b200_stream s);
 int gs_b200_dilate_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, unsigned n,
                          gs_b200_stream s);
+/* `iters` passes of gs_erode / gs_dilate (reference grayskull.h:285-304) in one call, as the reference CLI's
+ * `morph <op> <n>` verb (nanomagick.c:110-135) applies them: bit-identical to `iters` ping-ponged calls of
+ * gs_b200_erode_batch / gs_b200_dilate_batch, i.e. the min (max) over the in-image pixels of the
+ * (2*iters+1) x (2*iters+1) square.  Every dst byte is written; iters == 0 copies src to dst.  dst must not alias
+ * src.  The arithmetic per pixel grows at most logarithmically with iters (DESIGN.md §3, §6 for times).  With iters
+ * above 16, or geometry the TMA kernels cannot take, it uses library workspace of at most 256 MiB (or one frame, if
+ * a frame is larger). */
+int gs_b200_erode_n_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, unsigned n, unsigned iters,
+                          gs_b200_stream s);
+int gs_b200_dilate_n_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, unsigned n, unsigned iters,
+                           gs_b200_stream s);
 
 /* ---- resampling ------------------------------------------------------------------------- */
 /* gs_resize, reference grayskull.h:171-187 */
