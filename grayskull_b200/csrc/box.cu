@@ -491,7 +491,9 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
 //                that can occur, box_wide_magic_ok); clipped counts and r > 63 take
 //                floor(fdiv_rn(S, count)), which is exact for count < 2^17 and quotients <= 255 (the distance of
 //                S/count to the next integer is >= 1/count > half an ulp).
-template <bool ADAPTIVE, bool ALIGNED>
+// launch_box sends every frame with w % 8 == 0 and 8-byte aligned bases to k_box_mid, so this kernel only ever sees
+// ragged widths or unaligned bases: rows are gathered byte by byte and outputs stored byte by byte.
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(128)
 k_box_wide(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, int w, int h, int r, int R8, int BH,
            int strips, int cparam, float minv, int fast_ok) {
@@ -507,7 +509,7 @@ k_box_wide(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, int w, in
   const int yb = (int)blockIdx.y * BH, ye = min(h, yb + BH);
   const uint8_t *frame = src + (size_t)blockIdx.z * w * h;
   uint8_t *out = dst + (size_t)blockIdx.z * w * h;
-  const bool lane_in = ALIGNED ? (x0 >= 0 && x0 < w) : (x0 + 7 >= 0 && x0 < w);
+  const bool lane_in = x0 + 7 >= 0 && x0 < w;
   const bool out_lane = 8 * lane >= R8 && 8 * lane + 8 <= 256 - R8 && x0 < w && x0 + 7 >= 0;
   const int FULL = 2 * r + 1;
   // all 8 pixels of this lane have the full (2r+1)-column window inside the image
@@ -517,7 +519,6 @@ k_box_wide(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, int w, in
   // instructions in the first ncu capture)
   auto ldp = [&](const uint8_t *p, int y) -> uint2 {
     if (!lane_in || y < 0 || y >= h) return make_uint2(0u, 0u);
-    if (ALIGNED) return __ldg(reinterpret_cast<const uint2 *>(p));
     uint32_t a = 0, b = 0;
 #pragma unroll
     for (int k = 0; k < 4; k++) {
@@ -602,13 +603,9 @@ k_box_wide(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, int w, in
       uint2 o;
       o.x = q[0] | (q[1] << 8) | (q[2] << 16) | (q[3] << 24);
       o.y = q[4] | (q[5] << 8) | (q[6] << 16) | (q[7] << 24);
-      if (ALIGNED) {
-        st_cs_u2(qo, o);
-      } else {
 #pragma unroll
-        for (int k = 0; k < 8; k++)
-          if (x0 + k >= 0 && x0 + k < w) qo[k] = (uint8_t)((k < 4 ? o.x : o.y) >> (8 * (k & 3)));
-      }
+      for (int k = 0; k < 8; k++)
+        if (x0 + k >= 0 && x0 + k < w) qo[k] = (uint8_t)((k < 4 ? o.x : o.y) >> (8 * (k & 3)));
     }
     qo += w;
     // ---- roll the column sums down one row
@@ -1083,10 +1080,7 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
       GSB_LAUNCHED(1);
       return 0;
     }
-    if (aligned)
-      k_box_wide<ADAPTIVE, true><<<grid, 128, 0, s>>>(dst, src, (int)w, (int)h, (int)r, R8, BH, strips, cparam, minv, fast_ok);
-    else
-      k_box_wide<ADAPTIVE, false><<<grid, 128, 0, s>>>(dst, src, (int)w, (int)h, (int)r, R8, BH, strips, cparam, minv, fast_ok);
+    k_box_wide<ADAPTIVE><<<grid, 128, 0, s>>>(dst, src, (int)w, (int)h, (int)r, R8, BH, strips, cparam, minv, fast_ok);
     GSB_LAUNCHED(1);
     return 0;
   }

@@ -261,13 +261,14 @@ def _box_mid_row_model(C, r, R8, w_img, xs, look_ahead=True):
 def test_box_mid_row_walk_matches_direct_window_sums():
     """box.cu k_box_mid, H-phase index arithmetic (r mod 4 element positions, permuted pair layout, first / last groups,
     in-place output store, look-ahead guards) against direct window sums, for every radius the kernel takes and strips at
-    the left edge, in the interior and hanging over the right edge of the image"""
+    the left edge, in the interior and hanging over the right edge of the image.  r = 1..7 reach the kernel when a frame
+    fails the TMA kernel's 16-byte test (w = 8 mod 16, or a base 8 but not 16-byte aligned); widths 8 mod 16 included"""
     rng = np.random.default_rng(5)
-    for r in list(range(8, 41)) + [47, 48, 63, 64, 77, 100, 119, 120]:
+    for r in list(range(1, 41)) + [47, 48, 63, 64, 77, 100, 119, 120]:
         R8 = (r + 7) // 8 * 8
         outw = 256 - 2 * R8
         assert outw >= 16
-        for w_img in (outw * 3 + 40, 4096, 8 * ((r + 9) // 8)):
+        for w_img in (outw * 3 + 40, 4096, 8 * ((r + 9) // 8), 24, 200, 1080):
             strips = (w_img + outw - 1) // outw
             for strip in sorted({0, strips // 2, strips - 1}):
                 xs = strip * outw - R8
