@@ -437,25 +437,23 @@ int gs_b200_blobs_batch(const uint8_t *img, unsigned w, unsigned h, unsigned n, 
   GSB_CHECK(cudaMemsetAsync(bs.minx, 0xFF, 2 * sizeof(unsigned) * sn, st));          // minx, miny
   GSB_CHECK(cudaMemsetAsync(bs.maxx, 0, 4 * sizeof(unsigned) * sn, st));             // maxx, maxy, sx, sy
   const unsigned row_blocks = (unsigned)((rows_total + 7) / 8);
-  gsb::k_blob_mask<<<row_blocks, 256, 0, st>>>(img, w, h, mw, mask, rows_total);
-  gsb::k_blob_seed<<<row_blocks, 256, 0, st>>>(mask, h, mw, seed, sprefix, rowoff, rows_total);
-  gsb::k_row_scan<<<n, 1024, 0, st>>>(rowoff, h, totals, 0xFFFFFFFFu);
-  gsb::k_blob_overflow<<<(n + 63) / 64, 64, 0, st>>>(mask, seed, sprefix, rowoff, totals, h, mw, nblobs, n);
-  gsb::k_blob_runs<<<row_blocks, 256, 0, st>>>(mask, w, h, mw, parent, rows_total);
-  gsb::k_blob_union<<<(unsigned)((words_total + 255) / 256), 256, 0, st>>>(mask, w, h, mw, parent, words_total);
-  gsb::k_blob_label<<<(unsigned)((words_total + 7) / 8), 256, 0, st>>>(mask, seed, sprefix, rowoff, w, h, mw, parent, labels, bs,
-                                                                       nblobs, words_total);
-  gsb::k_blob_compact<<<n, 256, 0, st>>>(bs, totals, nblobs, reinterpret_cast<gsb::BlobRec *>(blobs), counts);
-  GSB_LAUNCHED(8);
+  GSB_LAUNCH(gsb::k_blob_mask, row_blocks, 256, 0, st, img, w, h, mw, mask, rows_total);
+  GSB_LAUNCH(gsb::k_blob_seed, row_blocks, 256, 0, st, mask, h, mw, seed, sprefix, rowoff, rows_total);
+  GSB_LAUNCH(gsb::k_row_scan, n, 1024, 0, st, rowoff, h, totals, 0xFFFFFFFFu);
+  GSB_LAUNCH(gsb::k_blob_overflow, (n + 63) / 64, 64, 0, st, mask, seed, sprefix, rowoff, totals, h, mw, nblobs, n);
+  GSB_LAUNCH(gsb::k_blob_runs, row_blocks, 256, 0, st, mask, w, h, mw, parent, rows_total);
+  GSB_LAUNCH(gsb::k_blob_union, (unsigned)((words_total + 255) / 256), 256, 0, st, mask, w, h, mw, parent, words_total);
+  GSB_LAUNCH(gsb::k_blob_label, (unsigned)((words_total + 7) / 8), 256, 0, st, mask, seed, sprefix, rowoff, w, h, mw, parent,
+             labels, bs, nblobs, words_total);
+  GSB_LAUNCH(gsb::k_blob_compact, n, 256, 0, st, bs, totals, nblobs, reinterpret_cast<gsb::BlobRec *>(blobs), counts);
   return 0;
 }
 
 int gs_b200_blob_corners(const uint8_t *img, unsigned w, unsigned h, const uint16_t *labels, const struct gs_blob *blob,
                          struct gs_point *corners, gs_b200_stream s) {
   GSB_ASSERT(img && w > 0 && h > 0 && blob && labels && corners);   // reference :409
-  gsb::k_blob_corners<<<1, 256, 0, static_cast<cudaStream_t>(s)>>>(img, w, h, labels, reinterpret_cast<const gsb::BlobRec *>(blob),
-                                                                   reinterpret_cast<unsigned *>(corners));
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_blob_corners, 1, 256, 0, static_cast<cudaStream_t>(s), img, w, h, labels,
+             reinterpret_cast<const gsb::BlobRec *>(blob), reinterpret_cast<unsigned *>(corners));
   return 0;
 }
 
@@ -470,8 +468,7 @@ int gs_b200_perspective_correct_batch(uint8_t *dst, unsigned dw, unsigned dh, co
   else
     for (int i = 0; i < 4; i++) q.x[i] = (float)corners[i].x, q.y[i] = (float)corners[i].y;   // 4 points in HOST memory
   dim3 grid((dw + 255) / 256, dh, n < 64u ? n : 64u);
-  gsb::k_perspective<<<grid, 256, 0, static_cast<cudaStream_t>(s)>>>(dst, dw, dh, src, sw, sh, n, dev, q);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_perspective, grid, 256, 0, static_cast<cudaStream_t>(s), dst, dw, dh, src, sw, sh, n, dev, q);
   return 0;
 }
 

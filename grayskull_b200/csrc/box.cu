@@ -995,22 +995,6 @@ __global__ void k_box_generic(uint8_t *__restrict__ dst, const uint8_t *__restri
   }
 }
 
-template <int R, bool ADAPTIVE>
-static int launch_box_r(const CUtensorMap &tmap, uint8_t *dst, unsigned w, unsigned h, unsigned n,
-                        int cparam, cudaStream_t s) {
-  // tile t covers output columns [240 t - 8, 240 t + 232)
-  const unsigned tiles_x = (w + 8 + BX_STRIDE - 1) / BX_STRIDE, tiles_y = (h + BX_TH - 1) / BX_TH;
-  GSB_ASSERT(tiles_y <= 65535u && n <= 65535u);   // grid y / z limits (launch_box checks n)
-  static DeviceOnce once;                         // per instantiation
-  if (once.needed()) {
-    GSB_CHECK(cudaFuncSetAttribute(k_box_tma<R, ADAPTIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, BX_SMEM));
-    once.done();
-  }
-  k_box_tma<R, ADAPTIVE><<<dim3(tiles_x, tiles_y, n), BX_THREADS, BX_SMEM, s>>>(tmap, dst, w, h, cparam);
-  GSB_LAUNCHED(1);
-  return 0;
-}
-
 template <bool ADAPTIVE>
 static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, unsigned n, unsigned r,
                       int cparam, cudaStream_t s) {
@@ -1018,15 +1002,14 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
   CUtensorMap tmap;
   if (r >= 1 && r <= BX_RMAX && tma_ok(src, w) && tma_ok(dst, w) &&
       n <= 65535u && make_tmap_u8frames(&tmap, src, w, h, n, BX_PW, BX_TH + 2 * r)) {
-    switch (r) {
-      case 1: return launch_box_r<1, ADAPTIVE>(tmap, dst, w, h, n, cparam, s);
-      case 2: return launch_box_r<2, ADAPTIVE>(tmap, dst, w, h, n, cparam, s);
-      case 3: return launch_box_r<3, ADAPTIVE>(tmap, dst, w, h, n, cparam, s);
-      case 4: return launch_box_r<4, ADAPTIVE>(tmap, dst, w, h, n, cparam, s);
-      case 5: return launch_box_r<5, ADAPTIVE>(tmap, dst, w, h, n, cparam, s);
-      case 6: return launch_box_r<6, ADAPTIVE>(tmap, dst, w, h, n, cparam, s);
-      default: return launch_box_r<7, ADAPTIVE>(tmap, dst, w, h, n, cparam, s);
-    }
+    static decltype(&k_box_tma<1, ADAPTIVE>) const box_tma_fn[BX_RMAX] = {
+        k_box_tma<1, ADAPTIVE>, k_box_tma<2, ADAPTIVE>, k_box_tma<3, ADAPTIVE>, k_box_tma<4, ADAPTIVE>,
+        k_box_tma<5, ADAPTIVE>, k_box_tma<6, ADAPTIVE>, k_box_tma<7, ADAPTIVE>};
+    // tile t covers output columns [240 t - 8, 240 t + 232)
+    const unsigned tiles_x = (w + 8 + BX_STRIDE - 1) / BX_STRIDE, tiles_y = (h + BX_TH - 1) / BX_TH;
+    GSB_ASSERT(tiles_y <= 65535u);   // grid y limit (z was checked above)
+    GSB_LAUNCH(box_tma_fn[r - 1], dim3(tiles_x, tiles_y, n), BX_THREADS, BX_SMEM, s, tmap, dst, w, h, cparam);
+    return 0;
   }
   if (r >= 1 && r <= 120 && !force_generic() && n <= 65535u && w < (1u << 30) && h < (1u << 30)) {
     // radius-independent path: warp-autonomous 256-column segments, u32 window sums (k_box_wide)
@@ -1061,46 +1044,17 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
       CUtensorMap pmap;
       const int use_tpf = make_tmap_u8frames(&pmap, src, w, h, n, 72, 32) ? 1 : 0;   // needs w % 16 == 0 and a 16-byte aligned base
       if (!use_tpf) memset(&pmap, 0, sizeof(pmap));
-      static DeviceOnce once;
-      if (once.needed()) {
-        GSB_CHECK(cudaFuncSetAttribute(k_box_mid<0, ADAPTIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, BM_SMEM));
-        GSB_CHECK(cudaFuncSetAttribute(k_box_mid<1, ADAPTIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, BM_SMEM));
-        GSB_CHECK(cudaFuncSetAttribute(k_box_mid<2, ADAPTIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, BM_SMEM));
-        GSB_CHECK(cudaFuncSetAttribute(k_box_mid<3, ADAPTIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, BM_SMEM));
-        once.done();
-      }
-#define GSB_BM_LAUNCH(RMV) k_box_mid<RMV, ADAPTIVE><<<grid, 32, BM_SMEM, s>>>(pmap, use_tpf, dst, src, (int)w, (int)h, (int)r, R8, BH, strips, cparam, minv, fast_ok)
-      switch (r & 3) {
-        case 0: GSB_BM_LAUNCH(0); break;
-        case 1: GSB_BM_LAUNCH(1); break;
-        case 2: GSB_BM_LAUNCH(2); break;
-        default: GSB_BM_LAUNCH(3); break;
-      }
-#undef GSB_BM_LAUNCH
-      GSB_LAUNCHED(1);
+      static decltype(&k_box_mid<0, ADAPTIVE>) const box_mid_fn[4] = {k_box_mid<0, ADAPTIVE>, k_box_mid<1, ADAPTIVE>,
+                                                                      k_box_mid<2, ADAPTIVE>, k_box_mid<3, ADAPTIVE>};
+      GSB_LAUNCH(box_mid_fn[r & 3], grid, 32, BM_SMEM, s, pmap, use_tpf, dst, src, (int)w, (int)h, (int)r, R8, BH, strips,
+                 cparam, minv, fast_ok);
       return 0;
     }
-    k_box_wide<ADAPTIVE><<<grid, 128, 0, s>>>(dst, src, (int)w, (int)h, (int)r, R8, BH, strips, cparam, minv, fast_ok);
-    GSB_LAUNCHED(1);
+    GSB_LAUNCH(k_box_wide<ADAPTIVE>, grid, 128, 0, s, dst, src, (int)w, (int)h, (int)r, R8, BH, strips, cparam, minv, fast_ok);
     return 0;
   }
   dim3 block(32, 8), grid((w + 31) / 32, (h + 7) / 8, n < 65535u ? n : 65535u);
-  k_box_generic<ADAPTIVE><<<grid, block, 0, s>>>(dst, src, w, h, n, r, cparam);
-  GSB_LAUNCHED(1);
-  return 0;
-}
-
-template <int R>
-static int launch_blur_sobel_r(const CUtensorMap &tmap, uint8_t *dst, unsigned w, unsigned h, unsigned n, cudaStream_t s) {
-  const unsigned tiles_x = (w + 8 + BS_STRIDE - 1) / BS_STRIDE, tiles_y = (h + BX_TH - 1) / BX_TH;
-  GSB_ASSERT(tiles_y <= 65535u && n <= 65535u);
-  static DeviceOnce once;
-  if (once.needed()) {
-    GSB_CHECK(cudaFuncSetAttribute(k_blur_sobel_tma<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, BS_SMEM));
-    once.done();
-  }
-  k_blur_sobel_tma<R><<<dim3(tiles_x, tiles_y, n), BX_THREADS, BS_SMEM, s>>>(tmap, dst, w, h);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(k_box_generic<ADAPTIVE>, grid, block, 0, s, dst, src, w, h, n, r, cparam);
   return 0;
 }
 
@@ -1115,15 +1069,13 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
   CUtensorMap tmap;
   if (radius >= 1 && radius <= gsb::BX_RMAX && gsb::tma_ok(src, w) && gsb::tma_ok(dst, w) && n <= 65535u &&
       gsb::make_tmap_u8frames(&tmap, src, w, h, n, gsb::BX_PW, gsb::BX_TH + 2 + 2 * radius)) {
-    switch (radius) {
-      case 1: return gsb::launch_blur_sobel_r<1>(tmap, dst, w, h, n, s);
-      case 2: return gsb::launch_blur_sobel_r<2>(tmap, dst, w, h, n, s);
-      case 3: return gsb::launch_blur_sobel_r<3>(tmap, dst, w, h, n, s);
-      case 4: return gsb::launch_blur_sobel_r<4>(tmap, dst, w, h, n, s);
-      case 5: return gsb::launch_blur_sobel_r<5>(tmap, dst, w, h, n, s);
-      case 6: return gsb::launch_blur_sobel_r<6>(tmap, dst, w, h, n, s);
-      default: return gsb::launch_blur_sobel_r<7>(tmap, dst, w, h, n, s);
-    }
+    static decltype(&gsb::k_blur_sobel_tma<1>) const blur_sobel_fn[gsb::BX_RMAX] = {
+        gsb::k_blur_sobel_tma<1>, gsb::k_blur_sobel_tma<2>, gsb::k_blur_sobel_tma<3>, gsb::k_blur_sobel_tma<4>,
+        gsb::k_blur_sobel_tma<5>, gsb::k_blur_sobel_tma<6>, gsb::k_blur_sobel_tma<7>};
+    const unsigned tiles_x = (w + 8 + gsb::BS_STRIDE - 1) / gsb::BS_STRIDE, tiles_y = (h + gsb::BX_TH - 1) / gsb::BX_TH;
+    GSB_ASSERT(tiles_y <= 65535u);
+    GSB_LAUNCH(blur_sobel_fn[radius - 1], dim3(tiles_x, tiles_y, n), gsb::BX_THREADS, gsb::BS_SMEM, s, tmap, dst, w, h);
+    return 0;
   }
   // other radii / ragged widths: the two per-op kernels through a scratch frame batch (same result, 4 B/px)
   uint8_t *tmp = static_cast<uint8_t *>(gsb::workspace(s, gsb::WS_STAGE_FUSED, (size_t)w * h * n));

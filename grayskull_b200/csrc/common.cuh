@@ -1,4 +1,4 @@
-// common.cuh -- shared plumbing of libgrayskull_b200.so: error recording, launch counting,
+// common.cuh -- shared plumbing of libgrayskull_b200.so: error recording, the kernel launch helper,
 // per-stream device workspace, TMA tensor maps and the mbarrier / bulk-tensor-copy PTX wrappers.
 #pragma once
 #include <cuda.h>
@@ -8,7 +8,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 
-#include <atomic>
+#include <utility>
 
 #include "../../include/grayskull_b200.h"
 
@@ -16,7 +16,6 @@ namespace gsb {
 
 // ---- host side ------------------------------------------------------------------------------
 int record_error(cudaError_t e, const char *file, int line);
-void count_launches(unsigned n);
 bool force_generic();  // GS_B200_FORCE_GENERIC=1: never take the TMA-tiled kernels (tests)
 int sm_count();        // SMs of the current device (grid sizing)
 
@@ -25,11 +24,29 @@ int sm_count();        // SMs of the current device (grid sizing)
     cudaError_t gsb_e_ = (expr);                                               \
     if (gsb_e_ != cudaSuccess) return gsb::record_error(gsb_e_, __FILE__, __LINE__); \
   } while (0)
-#define GSB_LAUNCHED(n)                 \
-  do {                                  \
-    gsb::count_launches(n);             \
-    GSB_CHECK(cudaGetLastError());      \
+
+// the two out-of-line halves of launch(): raise kernel k's dynamic shared-memory limit on the current device to at
+// least `smem` bytes (once per size it grows to), and count one launch and check it
+int opt_in_smem(const void *k, size_t smem, const char *file, int line);
+int launched(const char *file, int line);
+
+#ifdef __CUDACC__
+// Every kernel launch of the library: opt-in, launch, count, check.  The arguments convert to the kernel's own
+// parameter types exactly as in a direct <<<>>> call.  Returns 0 or the CUDA error (recorded at file:line).
+template <class... P, class... A>
+int launch(const char *file, int line, void (*k)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
+           A &&...a) {
+  if (smem)
+    if (int rc = opt_in_smem(reinterpret_cast<const void *>(k), smem, file, line)) return rc;
+  k<<<grid, block, smem, s>>>(std::forward<A>(a)...);
+  return launched(file, line);
+}
+#define GSB_LAUNCH(...)                                         \
+  do {                                                          \
+    int gsb_rc_ = gsb::launch(__FILE__, __LINE__, __VA_ARGS__); \
+    if (gsb_rc_) return gsb_rc_;                                \
   } while (0)
+#endif  // __CUDACC__
 
 // the reference's gs_assert (grayskull.h:94-98): message + abort
 #define GSB_ASSERT(cond)                                \
@@ -44,19 +61,6 @@ int sm_count();        // SMs of the current device (grid sizing)
 // exit: the hot path must not cudaMalloc per call.  Returns nullptr on allocation failure.
 void *workspace(cudaStream_t s, int slot, size_t bytes);
 
-// Per-device one-time setup at a call site (function attributes such as the dynamic shared-memory opt-in are
-// per device):   static DeviceOnce once;  if (once.needed()) { ...setup...; once.done(); }
-// Two threads racing on the same device may both run the setup, which is harmless; none skips it.
-struct DeviceOnce {
-  std::atomic<unsigned long long> mask{0};
-  static unsigned long long bit() {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    return 1ull << (dev & 63);
-  }
-  bool needed() const { return !(mask.load(std::memory_order_acquire) & bit()); }
-  void done() { mask.fetch_or(bit(), std::memory_order_release); }
-};
 enum { WS_INTEGRAL = 0, WS_FAST_A, WS_FAST_B, WS_ORB_A, WS_ORB_B, WS_LBP_A, WS_LBP_B, WS_LBP_C,
        WS_STAGE_A, WS_STAGE_B, WS_STAGE_C, WS_STAGE_D, WS_HIST, WS_STAGE_FUSED, WS_BLOB_A, WS_BLOB_B, WS_BLOB_C, WS_MORPH, WS_SLOTS };
 

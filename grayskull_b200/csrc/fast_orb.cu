@@ -49,9 +49,11 @@ static const uint32_t h_brief[256] = {
 // half-filled table
 static int brief_table_init() {
   static std::mutex mu;
-  static DeviceOnce once;
+  static bool filled[64];
+  int dev = 0;
+  GSB_CHECK(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lock(mu);
-  if (!once.needed()) return 0;
+  if (filled[dev & 63]) return 0;
   float4 t[256];
   for (int i = 0; i < 256; i++) {
     const uint32_t pk = h_brief[i];
@@ -59,7 +61,7 @@ static int brief_table_init() {
                        (float)(int)(int8_t)((pk >> 16) & 0xFF), (float)(int)(int8_t)(pk >> 24));
   }
   GSB_CHECK(cudaMemcpyToSymbol(c_brieff, t, sizeof(t)));
-  once.done();
+  filled[dev & 63] = true;
   return 0;
 }
 
@@ -894,8 +896,7 @@ static void trig_selfcheck_run() {
   cudaStream_t st = nullptr;
   if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) return;
   if (cudaMalloc(&dev, sizeof(host)) == cudaSuccess) {
-    k_trig_selfcheck<<<(TRIG_CHECK_N + 255) / 256, 256, 0, st>>>(dev);
-    count_launches(1);
+    (void)launch(__FILE__, __LINE__, k_trig_selfcheck, (TRIG_CHECK_N + 255) / 256, 256, 0, st, dev);
     if (cudaMemcpyAsync(host, dev, sizeof(host), cudaMemcpyDeviceToHost, st) == cudaSuccess &&
         cudaStreamSynchronize(st) == cudaSuccess) {
       int bad = 0;
@@ -950,32 +951,24 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
     GSB_ASSERT(grid.y <= 65535u);
     GSB_CHECK(cudaMemsetAsync(rowcount, 0, sizeof(unsigned) * (size_t)rows * n, s));
     CUtensorMap tmap;
-    if (tma_ok(src, w) && tma_ok(score, w) && make_tmap_u8frames(&tmap, src, w, h, n, FT_SW / 4, F2_SH))
-      k_fast_tiled2<true><<<grid, F2_THREADS, 0, s>>>(tmap, src, w, h, score, threshold, mw, masks, rowcount);
-    else {
-      memset(&tmap, 0, sizeof(tmap));
-      k_fast_tiled2<false><<<grid, F2_THREADS, 0, s>>>(tmap, src, w, h, score, threshold, mw, masks, rowcount);
-    }
-    GSB_LAUNCHED(1);
+    const bool tiled = tma_ok(src, w) && tma_ok(score, w) && make_tmap_u8frames(&tmap, src, w, h, n, FT_SW / 4, F2_SH);
+    if (!tiled) memset(&tmap, 0, sizeof(tmap));
+    GSB_LAUNCH(tiled ? k_fast_tiled2<true> : k_fast_tiled2<false>, grid, F2_THREADS, 0, s, tmap, src, w, h, score, threshold,
+               mw, masks, rowcount);
   } else {
     // foreign-sized score map (single-image gs_fast only), force_generic or t > 255: gs_set semantics per pixel,
     // then the NMS mask as a second pass
     dim3 block(32, 8), grid((w - 6 + 31) / 32, (h - 6 + 7) / 8, n);
-    k_fast_score<<<grid, block, 0, s>>>(src, w, h, n, score, sw, sh, threshold);
-    GSB_LAUNCHED(1);
-    if (sw % 4 == 0 && reinterpret_cast<uintptr_t>(score) % 4 == 0 && sw >= w && sh >= h)   // word pre-test stays inside the map
-      k_nms_mask<true><<<dim3((rows + 7) / 8, n), 256, 0, s>>>(score, sw, sh, w, h, mw, masks, rowcount);
-    else
-      k_nms_mask<false><<<dim3((rows + 7) / 8, n), 256, 0, s>>>(score, sw, sh, w, h, mw, masks, rowcount);
-    GSB_LAUNCHED(1);
+    GSB_LAUNCH(k_fast_score, grid, block, 0, s, src, w, h, n, score, sw, sh, threshold);
+    const bool words = sw % 4 == 0 && reinterpret_cast<uintptr_t>(score) % 4 == 0 && sw >= w && sh >= h;   // word pre-test stays inside the map
+    GSB_LAUNCH(words ? k_nms_mask<true> : k_nms_mask<false>, dim3((rows + 7) / 8, n), 256, 0, s, score, sw, sh, w, h, mw, masks,
+               rowcount);
   }
-  k_row_scan<<<n, 1024, 0, s>>>(rowcount, rows, counts, nkps);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(k_row_scan, n, 1024, 0, s, rowcount, rows, counts, nkps);
   const unsigned long long rows_total = (unsigned long long)rows * n;
   GSB_ASSERT(rows_total < 0x7FFFFFFFull);
-  k_nms_emit_masks<<<(unsigned)((rows_total + 7) / 8), 256, 0, s>>>(score, sw, sh, w, h, mw, masks, rowcount,
-                                                                    (unsigned)rows_total, kps, nkps);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(k_nms_emit_masks, (unsigned)((rows_total + 7) / 8), 256, 0, s, score, sw, sh, w, h, mw, masks, rowcount,
+             (unsigned)rows_total, kps, nkps);
   return 0;
 }
 
@@ -1011,21 +1004,18 @@ int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsign
   if (!cand || !ccount) return (int)cudaErrorMemoryAllocation;
   int rc = gsb::fast_impl(src, w, h, n, scoremap, w, h, cand, ccount, cap, threshold, st);
   if (rc) return rc;
-  gsb::k_orb_select<<<n, 256, 0, st>>>(cand, ccount, cap, w, h, reinterpret_cast<gsb::KpRec *>(kps), counts, nkps);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_orb_select, n, 256, 0, st, cand, ccount, cap, w, h, reinterpret_cast<gsb::KpRec *>(kps), counts, nkps);
   const unsigned long long warps = (unsigned long long)n * nkps;
   const unsigned long long blocks = (warps + 7) / 8;
   GSB_ASSERT(blocks < 0x7FFFFFFFull);
   gsb::KpRec *kr = reinterpret_cast<gsb::KpRec *>(kps);
   if (gsb::g_trig_mode == 0) gsb::trig_selfcheck_once(st);
-  gsb::k_orb_moments<<<(unsigned)blocks, 256, 0, st>>>(src, w, h, kr, counts, nkps, n);
-  gsb::k_orb_trig<<<(unsigned)((warps + 255) / 256), 256, 0, st>>>(kr, counts, nkps, n, gsb::g_trig_mode);
+  GSB_LAUNCH(gsb::k_orb_moments, (unsigned)blocks, 256, 0, st, src, w, h, kr, counts, nkps, n);
+  GSB_LAUNCH(gsb::k_orb_trig, (unsigned)((warps + 255) / 256), 256, 0, st, kr, counts, nkps, n, gsb::g_trig_mode);
   if (int rcb = gsb::brief_table_init()) return rcb;
-  if (w % 4 == 0 && reinterpret_cast<uintptr_t>(src) % 4 == 0 && !gsb::force_generic())
-    gsb::k_orb_brief<true><<<(unsigned)blocks, 256, 0, st>>>(src, w, h, kr, counts, nkps, n);
-  else
-    gsb::k_orb_brief<false><<<(unsigned)blocks, 256, 0, st>>>(src, w, h, kr, counts, nkps, n);
-  GSB_LAUNCHED(3);
+  const bool words = w % 4 == 0 && reinterpret_cast<uintptr_t>(src) % 4 == 0 && !gsb::force_generic();
+  GSB_LAUNCH(words ? gsb::k_orb_brief<true> : gsb::k_orb_brief<false>, (unsigned)blocks, 256, 0, st, src, w, h, kr, counts, nkps,
+             n);
   return 0;
 }
 
@@ -1036,14 +1026,12 @@ int gsb_fast_single(const uint8_t *src, unsigned w, unsigned h, uint8_t *score, 
 }
 int gsb_orient_single(const uint8_t *img, unsigned w, unsigned x, unsigned y, unsigned r, float *out, cudaStream_t s) {
   if (gsb::g_trig_mode == 0) gsb::trig_selfcheck_once(s);
-  gsb::k_orient_one<<<1, 32, 0, s>>>(img, w, x, y, r, gsb::g_trig_mode, out);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_orient_one, 1, 32, 0, s, img, w, x, y, r, gsb::g_trig_mode, out);
   return 0;
 }
 int gsb_brief_single(const uint8_t *img, unsigned w, unsigned h, struct gs_keypoint *kp, cudaStream_t s) {
   if (gsb::g_trig_mode == 0) gsb::trig_selfcheck_once(s);
-  gsb::k_brief_one<<<1, 32, 0, s>>>(img, w, h, reinterpret_cast<gsb::KpRec *>(kp), gsb::g_trig_mode);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_brief_one, 1, 32, 0, s, img, w, h, reinterpret_cast<gsb::KpRec *>(kp), gsb::g_trig_mode);
   return 0;
 }
 }

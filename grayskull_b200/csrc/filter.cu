@@ -264,10 +264,9 @@ int gs_b200_filter_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned 
     if (norm == 1 || magic_ok) {
       dim3 grid((w / 8 + 31) / 32, (h + 8 * gsb::F3_ROWS - 1) / (8 * gsb::F3_ROWS), zn);
       GSB_ASSERT(grid.y <= 65535u);
-      if (norm == 1) gsb::k_filter3<true><<<grid, 256, 0, st>>>(dst, src, w, h, n, kr[0], kr[1], kr[2], 0);
-      else gsb::k_filter3<false><<<grid, 256, 0, st>>>(dst, src, w, h, n, kr[0], kr[1], kr[2],
-                                                       (uint32_t)((1ull << 32) / norm + 1));
-      GSB_LAUNCHED(1);
+      const uint32_t magic = norm == 1 ? 0 : (uint32_t)((1ull << 32) / norm + 1);
+      GSB_LAUNCH(norm == 1 ? gsb::k_filter3<true> : gsb::k_filter3<false>, grid, 256, 0, st, dst, src, w, h, n, kr[0], kr[1],
+                 kr[2], magic);
       return 0;
     }
   }
@@ -277,8 +276,7 @@ int gs_b200_filter_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned 
   if (kbytes) GSB_CHECK(cudaMemcpyAsync(dk, kernel, kbytes, cudaMemcpyHostToDevice, st));
   dim3 grid((w + 31) / 32, (h + 7) / 8, zn);
   GSB_ASSERT(grid.y <= 65535u);
-  gsb::k_filter_generic<<<grid, 256, 0, st>>>(dst, src, w, h, n, dk, has_kernel ? kw : 0, has_kernel ? kh : 0, norm);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_filter_generic, grid, 256, 0, st, dst, src, w, h, n, dk, has_kernel ? kw : 0, has_kernel ? kh : 0, norm);
   return 0;
 }
 
@@ -294,16 +292,14 @@ int gs_b200_match_template_batch(uint8_t *result, const uint8_t *img, unsigned w
     const unsigned twords = (tw + 3) / 4;
     uint32_t *tpack = static_cast<uint32_t *>(gsb::workspace(st, gsb::WS_HIST, sizeof(uint32_t) * (size_t)twords * th));
     if (!tpack) return (int)cudaErrorMemoryAllocation;
-    gsb::k_pack_template<<<(twords * th + 255) / 256, 256, 0, st>>>(tpack, tmpl, tw, th, twords);
+    GSB_LAUNCH(gsb::k_pack_template, (twords * th + 255) / 256, 256, 0, st, tpack, tmpl, tw, th, twords);
     dim3 grid(((rw + 3) / 4 + 31) / 32, (rh + 7) / 8, zn);
     GSB_ASSERT(grid.y <= 65535u);
-    gsb::k_match_template<<<grid, 256, 0, st>>>(result, img, w, h, n, tpack, tw, th, twords);
-    GSB_LAUNCHED(2);
+    GSB_LAUNCH(gsb::k_match_template, grid, 256, 0, st, result, img, w, h, n, tpack, tw, th, twords);
   } else {
     dim3 grid((rw + 31) / 32, (rh + 7) / 8, zn);
     GSB_ASSERT(grid.y <= 65535u);
-    gsb::k_match_template_generic<<<grid, 256, 0, st>>>(result, img, w, h, n, tmpl, tw, th);
-    GSB_LAUNCHED(1);
+    GSB_LAUNCH(gsb::k_match_template_generic, grid, 256, 0, st, result, img, w, h, n, tmpl, tw, th);
   }
   return 0;
 }
@@ -320,9 +316,8 @@ int gs_b200_find_best_match_batch(struct gs_point *best, const uint8_t *result, 
   if (!keys) return (int)cudaErrorMemoryAllocation;
   GSB_CHECK(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * n, st));
   dim3 grid((unsigned)((px + gsb::BM_CHUNK - 1) / gsb::BM_CHUNK), n);
-  gsb::k_best_match_partial<<<grid, 256, 0, st>>>(keys, result, px);
-  gsb::k_best_match_final<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<unsigned *>(best), keys, rw, n);
-  GSB_LAUNCHED(2);
+  GSB_LAUNCH(gsb::k_best_match_partial, grid, 256, 0, st, keys, result, px);
+  GSB_LAUNCH(gsb::k_best_match_final, (n + 127) / 128, 128, 0, st, reinterpret_cast<unsigned *>(best), keys, rw, n);
   return 0;
 }
 }

@@ -186,9 +186,7 @@ static int threshold_launch(uint8_t *img, unsigned w, unsigned h, unsigned n, co
     dim3 grid(gx, nf);
     uint8_t *p = img + (size_t)f0 * px;
     const uint8_t *tp = thresh ? thresh + f0 : nullptr;
-    if (vec) k_threshold<true><<<grid, 256, 0, st>>>(p, px, tp, scalar, offset);
-    else k_threshold<false><<<grid, 256, 0, st>>>(p, px, tp, scalar, offset);
-    GSB_LAUNCHED(1);
+    GSB_LAUNCH(vec ? k_threshold<true> : k_threshold<false>, grid, 256, 0, st, p, px, tp, scalar, offset);
   }
   return 0;
 }
@@ -209,22 +207,11 @@ int gs_b200_histogram_batch(unsigned *hist, const uint8_t *src, unsigned w, unsi
   unsigned cpf = (unsigned)((px + chunk - 1) / chunk);
   GSB_ASSERT((unsigned long long)cpf * n < 0xFFFFFFFFull);
   const unsigned units = cpf * n;
-  static int sm_counts[64] = {0};                // per device: SM count, and "shared-memory opt-in done"
-  int dev = 0;
-  GSB_CHECK(cudaGetDevice(&dev));
-  GSB_ASSERT(dev >= 0 && dev < 64);
-  if (!sm_counts[dev]) {
-    int sms = 0;
-    GSB_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    GSB_CHECK(cudaFuncSetAttribute(gsb::k_histogram<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gsb::HG_SMEM));
-    GSB_CHECK(cudaFuncSetAttribute(gsb::k_histogram<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, gsb::HG_SMEM));
-    sm_counts[dev] = sms;
-  }
-  const unsigned grid = units < (unsigned)sm_counts[dev] ? units : (unsigned)sm_counts[dev];
+  const unsigned sms = (unsigned)gsb::sm_count();
+  const unsigned grid = units < sms ? units : sms;
   const bool vec = px % 16 == 0 && reinterpret_cast<uintptr_t>(src) % 16 == 0;
-  if (vec) gsb::k_histogram<true><<<grid, gsb::HG_THREADS, gsb::HG_SMEM, st>>>(hist, src, px, units, cpf, chunk);
-  else gsb::k_histogram<false><<<grid, gsb::HG_THREADS, gsb::HG_SMEM, st>>>(hist, src, px, units, cpf, chunk);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(vec ? gsb::k_histogram<true> : gsb::k_histogram<false>, grid, gsb::HG_THREADS, gsb::HG_SMEM, st, hist, src, px,
+             units, cpf, chunk);
   return 0;
 }
 
@@ -239,8 +226,7 @@ int gs_b200_otsu_threshold_batch(uint8_t *thresh, unsigned *hist, const uint8_t 
   }
   int rc = gs_b200_histogram_batch(hist, src, w, h, n, s);
   if (rc) return rc;
-  gsb::k_otsu<<<(n + 3) / 4, 128, 0, st>>>(thresh, hist, w * h, n);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_otsu, (n + 3) / 4, 128, 0, st, thresh, hist, w * h, n);
   return 0;
 }
 

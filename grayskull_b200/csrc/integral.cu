@@ -326,13 +326,9 @@ extern "C" int gs_b200_integral_batch(uint32_t *ii, const uint8_t *src, unsigned
       unsigned char *ws = static_cast<unsigned char *>(gsb::workspace(st, gsb::WS_INTEGRAL, 256 + slot_bytes));
       if (!ws) return (int)cudaErrorMemoryAllocation;
       GSB_CHECK(cudaMemsetAsync(ws, 0, 256 + (strips > 1 ? slot_bytes : 0), st));
-      if (narrow)
-        gsb::k_integral_strips<64, 16><<<(unsigned)ctas, 64, 0, st>>>(ii, src, w, h, n, strips, nbands, reinterpret_cast<unsigned *>(ws),
-                                                                     reinterpret_cast<unsigned long long *>(ws + 256));
-      else
-        gsb::k_integral_strips<128, 8><<<(unsigned)ctas, 128, 0, st>>>(ii, src, w, h, n, strips, nbands, reinterpret_cast<unsigned *>(ws),
-                                                                      reinterpret_cast<unsigned long long *>(ws + 256));
-      GSB_LAUNCHED(1);
+      GSB_LAUNCH(narrow ? gsb::k_integral_strips<64, 16> : gsb::k_integral_strips<128, 8>, (unsigned)ctas, narrow ? 64 : 128, 0,
+                 st, ii, src, w, h, n, strips, nbands, reinterpret_cast<unsigned *>(ws),
+                 reinterpret_cast<unsigned long long *>(ws + 256));
       return 0;
     }
   }
@@ -345,26 +341,16 @@ extern "C" int gs_b200_integral_batch(uint32_t *ii, const uint8_t *src, unsigned
     GSB_CHECK(cudaMemsetAsync(ctrl, 0, ctrl_bytes, st));
     const unsigned threads = ((w / 8 + 31) / 32) * 32;
     const size_t smem = sizeof(uint32_t) * gsb::IB_BH * threads;   // <= 64 KB
-    static gsb::DeviceOnce once;
-    if (once.needed()) {
-      GSB_CHECK(cudaFuncSetAttribute(gsb::k_integral_bands<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-      GSB_CHECK(cudaFuncSetAttribute(gsb::k_integral_bands<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-      once.done();
-    }
-    if (threads <= 512) gsb::k_integral_bands<512><<<n * nbands, threads, smem, st>>>(ii, src, w, h, n, nbands, ctrl);
-    else gsb::k_integral_bands<1024><<<n * nbands, threads, smem, st>>>(ii, src, w, h, n, nbands, ctrl);
-    GSB_LAUNCHED(1);
+    GSB_LAUNCH(threads <= 512 ? gsb::k_integral_bands<512> : gsb::k_integral_bands<1024>, n * nbands, threads, smem, st, ii,
+               src, w, h, n, nbands, ctrl);
     return 0;
   }
   const unsigned long long rows = (unsigned long long)h * n;
   const unsigned blocks = (unsigned)((rows + 7) / 8);
   const bool vec = (w % 4 == 0) && reinterpret_cast<uintptr_t>(src) % 4 == 0 &&
                    reinterpret_cast<uintptr_t>(ii) % 16 == 0;
-  if (vec) gsb::k_integral_rows<true><<<blocks, 256, 0, st>>>(ii, src, w, h, n);
-  else gsb::k_integral_rows<false><<<blocks, 256, 0, st>>>(ii, src, w, h, n);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(vec ? gsb::k_integral_rows<true> : gsb::k_integral_rows<false>, blocks, 256, 0, st, ii, src, w, h, n);
   dim3 grid((w + 127) / 128, n < 65535u ? n : 65535u);
-  gsb::k_integral_cols<<<grid, 128, 0, st>>>(ii, w, h, n);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_integral_cols, grid, 128, 0, st, ii, w, h, n);
   return 0;
 }

@@ -926,13 +926,8 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
   // k_lbp_scan3 (TMA-staged parity-plane tiles, warp-autonomous survivor lists) when the scan is the usual
   // step-2 one on 8-px-aligned tables; bit-exact with k_lbp_scan2, half its instructions.
   const bool v3 = !p->tiles.empty() && reinterpret_cast<uintptr_t>(ii) % 16 == 0 && !gsb::force_generic();
+  const bool v2 = !v3 && dc.safe_geometry && smem2 <= 160 * 1024 && (unsigned long long)iw * ih < 0x7FFFFFFFull;
   if (v3) {
-    static gsb::DeviceOnce once3;
-    if (once3.needed()) {
-      GSB_CHECK(cudaFuncSetAttribute(gsb::k_lbp_scan3<gsb::LBP3_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-      GSB_CHECK(cudaFuncSetAttribute(gsb::k_lbp_scan3<gsb::LBP3_BIG_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-      once3.done();
-    }
     GSB_CHECK(cudaMemsetAsync(masks, 0, 4 * (size_t)dc.total_slots * n, st));   // padding slots between scales
     // frames go through in chunks so that the de-interleaved copy stays small (<= 1 GiB of workspace)
     const size_t frame_bytes = (size_t)iw * ih * 4;
@@ -945,51 +940,29 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
       const unsigned nf = n - f0 < chunk ? n - f0 : chunk;
       const uint32_t *src = ii + (size_t)f0 * iw * ih;
       const size_t groups = (size_t)iw / 8 * ih;
-      gsb::k_deinterleave2<<<dim3((unsigned)((groups + 255) / 256), nf < 64u ? nf : 64u), 256, 0, st>>>(planes, src, iw, ih, nf);
-      GSB_LAUNCHED(1);
+      GSB_LAUNCH(gsb::k_deinterleave2, dim3((unsigned)((groups + 255) / 256), nf < 64u ? nf : 64u), 256, 0, st, planes, src,
+                 iw, ih, nf);
       for (int si = 0; si < dc.nscales; si++) {
         const gsb::TilePlan &tp = p->tiles[si];
         CUtensorMap tm;
         if (!gsb::make_tmap_u32frames(&tm, planes, iw / 2, ih, 2 * nf, (unsigned)tp.bw, (unsigned)tp.ph))
           return gsb::record_error(cudaErrorInvalidValue, __FILE__, __LINE__);
-        if (tp.threads == gsb::LBP3_BIG_THREADS)
-          gsb::k_lbp_scan3<gsb::LBP3_BIG_THREADS><<<dim3((unsigned)(tp.tiles_x * tp.tiles_y), nf), gsb::LBP3_BIG_THREADS, tp.smem, st>>>(
-              tm, dc, si, tp.twx, tp.twy, tp.bw, tp.ph, tp.tiles_x, gsb::LBP3_FLAT, 0, masks + (size_t)f0 * dc.total_slots);
-        else
-          gsb::k_lbp_scan3<gsb::LBP3_THREADS><<<dim3((unsigned)(tp.tiles_x * tp.tiles_y), nf), gsb::LBP3_THREADS, tp.smem, st>>>(
-              tm, dc, si, tp.twx, tp.twy, tp.bw, tp.ph, tp.tiles_x, gsb::LBP3_FLAT, 0, masks + (size_t)f0 * dc.total_slots);
-        GSB_LAUNCHED(1);
+        const bool big = tp.threads == gsb::LBP3_BIG_THREADS;
+        GSB_LAUNCH(big ? gsb::k_lbp_scan3<gsb::LBP3_BIG_THREADS> : gsb::k_lbp_scan3<gsb::LBP3_THREADS>,
+                   dim3((unsigned)(tp.tiles_x * tp.tiles_y), nf), big ? gsb::LBP3_BIG_THREADS : gsb::LBP3_THREADS, tp.smem, st,
+                   tm, dc, si, tp.twx, tp.twy, tp.bw, tp.ph, tp.tiles_x, gsb::LBP3_FLAT, 0, masks + (size_t)f0 * dc.total_slots);
       }
     }
-    gsb::k_lbp_count<<<dim3((unsigned)((nblocks + 255) / 256), n), 256, 0, st>>>(masks, dc.total_slots, bcount);
-    GSB_LAUNCHED(1);
-    gsb::k_row_scan<<<n, 1024, 0, st>>>(bcount, (unsigned)nblocks, counts, max_rects);
-    GSB_LAUNCHED(1);
-    gsb::k_lbp_emit<<<dim3((unsigned)((nblocks + 7) / 8), n), 256, 0, st>>>(dc, masks, bcount, counts, rects, max_rects);
-    GSB_LAUNCHED(1);
-    return 0;
-  }
-  const bool v2 = dc.safe_geometry && smem2 <= 160 * 1024 && (unsigned long long)iw * ih < 0x7FFFFFFFull;
-  if (v2) {
-    static gsb::DeviceOnce once2;
-    if (once2.needed()) {                         // the v2 condition above caps smem2 at 160 KB
-      GSB_CHECK(cudaFuncSetAttribute(gsb::k_lbp_scan2, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-      once2.done();
-    }
+  } else if (v2) {
     dim3 grid2((unsigned)(dc.total_slots / gsb::LBP_SLOTS_PER_CTA), n);
-    gsb::k_lbp_scan2<<<grid2, gsb::LBP_THREADS, smem2, st>>>(ii, iw, ih, dc, masks);
-    GSB_LAUNCHED(1);
-    gsb::k_lbp_count<<<dim3((unsigned)((nblocks + 255) / 256), n), 256, 0, st>>>(masks, dc.total_slots, bcount);
-  } else if (dc.safe_geometry) {
-    gsb::k_lbp_scan<false><<<grid, 256, 0, st>>>(ii, iw, ih, dc, masks, bcount);
+    GSB_LAUNCH(gsb::k_lbp_scan2, grid2, gsb::LBP_THREADS, smem2, st, ii, iw, ih, dc, masks);
   } else {
-    gsb::k_lbp_scan<true><<<grid, 256, 0, st>>>(ii, iw, ih, dc, masks, bcount);
+    GSB_LAUNCH(dc.safe_geometry ? gsb::k_lbp_scan<false> : gsb::k_lbp_scan<true>, grid, 256, 0, st, ii, iw, ih, dc, masks, bcount);
   }
-  GSB_LAUNCHED(1);
-  gsb::k_row_scan<<<n, 1024, 0, st>>>(bcount, (unsigned)nblocks, counts, max_rects);
-  GSB_LAUNCHED(1);
-  gsb::k_lbp_emit<<<dim3((unsigned)((nblocks + 7) / 8), n), 256, 0, st>>>(dc, masks, bcount, counts, rects, max_rects);
-  GSB_LAUNCHED(1);
+  if (v3 || v2)   // k_lbp_scan counts its blocks' survivors itself
+    GSB_LAUNCH(gsb::k_lbp_count, dim3((unsigned)((nblocks + 255) / 256), n), 256, 0, st, masks, dc.total_slots, bcount);
+  GSB_LAUNCH(gsb::k_row_scan, n, 1024, 0, st, bcount, (unsigned)nblocks, counts, max_rects);
+  GSB_LAUNCH(gsb::k_lbp_emit, dim3((unsigned)((nblocks + 7) / 8), n), 256, 0, st, dc, masks, bcount, counts, rects, max_rects);
   return 0;
 }
 
@@ -1025,11 +998,9 @@ int gsb_lbp_window_single(const struct gs_lbp_cascade *c, const uint32_t *ii, un
   GSB_CHECK(cudaMemcpyAsync(blob + o_sb, c->subsets, 4 * (size_t)nsub, cudaMemcpyHostToDevice, s));
   GSB_CHECK(cudaMemcpyAsync(blob + o_st, stages.data(), sizeof(gsb::Stage) * nst, cudaMemcpyHostToDevice, s));
   GSB_CHECK(cudaStreamSynchronize(s));  // the host vectors above go out of scope
-  gsb::k_lbp_window_one<<<1, 32, 0, s>>>(ii, iw, ih, x, y, reinterpret_cast<const short4 *>(blob + o_ft),
-                                         reinterpret_cast<const gsb::Weak *>(blob + o_wk),
-                                         reinterpret_cast<const int *>(blob + o_sb),
-                                         reinterpret_cast<const gsb::Stage *>(blob + o_st), nst, out_dev);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(gsb::k_lbp_window_one, 1, 32, 0, s, ii, iw, ih, x, y, reinterpret_cast<const short4 *>(blob + o_ft),
+             reinterpret_cast<const gsb::Weak *>(blob + o_wk), reinterpret_cast<const int *>(blob + o_sb),
+             reinterpret_cast<const gsb::Stage *>(blob + o_st), nst, out_dev);
   return 0;
 }
 }

@@ -306,9 +306,8 @@ static int morph_tma_step(uint8_t *dst, const uint8_t *src, unsigned w, unsigned
   const unsigned tiles_x = (w + MT_TW - 1) / MT_TW, tiles_y = (h + MT_TH - 1) / MT_TH;
   const unsigned long long blocks = (unsigned long long)tiles_x * tiles_y * n;
   GSB_ASSERT(blocks < 0x7FFFFFFFull);
-  morph_tma_fn<OP>(k, std::make_integer_sequence<int, MT_MAX_N - 1>())
-      <<<(unsigned)blocks, MT_THREADS, 0, s>>>(tmap, dst, w, h, tiles_x, tiles_y);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(morph_tma_fn<OP>(k, std::make_integer_sequence<int, MT_MAX_N - 1>()), (unsigned)blocks, MT_THREADS, 0, s, tmap,
+             dst, w, h, tiles_x, tiles_y);
   return 0;
 }
 
@@ -367,11 +366,10 @@ static int launch_morph_n(uint8_t *dst, const uint8_t *src, unsigned w, unsigned
     const unsigned long long rows = (unsigned long long)c * h, cols = (unsigned long long)c * w;
     const unsigned long long rblocks = (rows + RP_WARPS * 32 - 1) / (RP_WARPS * 32);
     GSB_ASSERT(rblocks < 0x7FFFFFFFull);
-    k_morph_rows<OP><<<(unsigned)rblocks, RP_WARPS * 32, 0, s>>>(ws, src + f0 * fb, w, nx, rows);
+    GSB_LAUNCH(k_morph_rows<OP>, (unsigned)rblocks, RP_WARPS * 32, 0, s, ws, src + f0 * fb, w, nx, rows);
     const unsigned long long ctotal = ((h - 1) / (2ull * ny + 1) + 1) * cols;
     const unsigned cblocks = (unsigned)min((ctotal + 255) / 256, (unsigned long long)sm_count() * 64);
-    k_morph_cols<OP><<<cblocks, 256, 0, s>>>(dst + f0 * fb, ws, w, h, ny, cols);
-    GSB_LAUNCHED(2);
+    GSB_LAUNCH(k_morph_cols<OP>, cblocks, 256, 0, s, dst + f0 * fb, ws, w, h, ny, cols);
   }
   return 0;
 }

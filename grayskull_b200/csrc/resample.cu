@@ -252,12 +252,11 @@ int gs_b200_downsample_batch(uint8_t *dst, const uint8_t *src, unsigned sw, unsi
   const unsigned zn = n < 65535u ? n : 65535u;
   if (gsb::tma_ok(src, sw) && reinterpret_cast<uintptr_t>(dst) % 8 == 0 && dh <= 65535u) {
     dim3 block(128), grid((dw / 8 + 127) / 128, dh, zn);
-    gsb::k_downsample_vec<<<grid, block, 0, st>>>(dst, src, sw, sh, dw, dh, n);
+    GSB_LAUNCH(gsb::k_downsample_vec, grid, block, 0, st, dst, src, sw, sh, dw, dh, n);
   } else {
     dim3 block(32, 8), grid((dw + 31) / 32, (dh + 7) / 8, zn);
-    gsb::k_downsample_generic<<<grid, block, 0, st>>>(dst, src, sw, sh, dw, dh, n);
+    GSB_LAUNCH(gsb::k_downsample_generic, grid, block, 0, st, dst, src, sw, sh, dw, dh, n);
   }
-  GSB_LAUNCHED(1);
   return 0;
 }
 
@@ -287,25 +286,13 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
     CUtensorMap tm;
     if (bytes <= (size_t)gsb::RT_MAX_BYTES && pitch <= 1024 && rows <= 256 && !pairs_case &&
         gsb::tma_ok(src, sw) && n <= 65535u && gsb::make_tmap_u8frames(&tm, src, sw, sh, n, pitch / 4, rows)) {
-      static gsb::DeviceOnce once;
-      if (once.needed()) {
-        GSB_CHECK(cudaFuncSetAttribute(gsb::k_resize_tiled<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gsb::RT_MAX_BYTES));
-        GSB_CHECK(cudaFuncSetAttribute(gsb::k_resize_tiled<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, gsb::RT_MAX_BYTES));
-        once.done();
-      }
-      if (vec_dst)
-        gsb::k_resize_tiled<true><<<grid, 256, bytes, static_cast<cudaStream_t>(s)>>>(tm, dst, dw, dh, sw, sh, n, pitch, rows);
-      else
-        gsb::k_resize_tiled<false><<<grid, 256, bytes, static_cast<cudaStream_t>(s)>>>(tm, dst, dw, dh, sw, sh, n, pitch, rows);
-      GSB_LAUNCHED(1);
+      GSB_LAUNCH(vec_dst ? gsb::k_resize_tiled<true> : gsb::k_resize_tiled<false>, grid, 256, bytes, static_cast<cudaStream_t>(s),
+                 tm, dst, dw, dh, sw, sh, n, pitch, rows);
       return 0;
     }
   }
-  if (vec_dst)
-    gsb::k_resize<true><<<grid, 256, 0, static_cast<cudaStream_t>(s)>>>(dst, dw, dh, src, sw, sh, n, aligned8);
-  else
-    gsb::k_resize<false><<<grid, 256, 0, static_cast<cudaStream_t>(s)>>>(dst, dw, dh, src, sw, sh, n, aligned8);
-  GSB_LAUNCHED(1);
+  GSB_LAUNCH(vec_dst ? gsb::k_resize<true> : gsb::k_resize<false>, grid, 256, 0, static_cast<cudaStream_t>(s), dst, dw, dh, src,
+             sw, sh, n, aligned8);
   return 0;
 }
 }

@@ -1,4 +1,4 @@
-// runtime.cu -- host runtime of libgrayskull_b200.so: error text, launch counter, workspace
+// runtime.cu -- host runtime of libgrayskull_b200.so: error text, launch counter and shared-memory opt-in, workspace
 // arenas, tensor-map construction (driver entry point fetched at run time, so the library links
 // against cudart only and loads on machines without a GPU driver), memory helpers of the C ABI.
 #include <atomic>
@@ -19,7 +19,28 @@ int record_error(cudaError_t e, const char *file, int line) {
            cudaGetErrorString(e), file, line);
   return static_cast<int>(e);
 }
-void count_launches(unsigned n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+// largest dynamic shared memory each (device, kernel) has been opted in to
+static std::mutex g_smem_mutex;
+static std::map<std::pair<int, const void *>, size_t> g_smem_optin;
+
+int opt_in_smem(const void *k, size_t smem, const char *file, int line) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return record_error(e, file, line);
+  std::lock_guard<std::mutex> lock(g_smem_mutex);
+  size_t &have = g_smem_optin[std::make_pair(dev, k)];
+  if (have >= smem) return 0;
+  e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e != cudaSuccess) return record_error(e, file, line);
+  have = smem;
+  return 0;
+}
+int launched(const char *file, int line) {
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : record_error(e, file, line);
+}
 
 static int g_force_generic = -1;
 bool force_generic() {

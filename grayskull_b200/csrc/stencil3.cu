@@ -205,12 +205,11 @@ static int launch_stencil3(uint8_t *dst, const uint8_t *src, unsigned w, unsigne
     const unsigned tiles_x = (w + S3_TW - 1) / S3_TW, tiles_y = (h + S3_TH - 1) / S3_TH;
     const unsigned long long blocks = (unsigned long long)tiles_x * tiles_y * n;
     GSB_ASSERT(blocks < 0x7FFFFFFFull);
-    k_stencil3_tma<OP><<<(unsigned)blocks, S3_WARPS * 32, 0, s>>>(tmap, dst, w, h, tiles_x, tiles_y);
+    GSB_LAUNCH(k_stencil3_tma<OP>, (unsigned)blocks, S3_WARPS * 32, 0, s, tmap, dst, w, h, tiles_x, tiles_y);
   } else {
     dim3 block(32, 8), grid((w + 31) / 32, (h + 7) / 8, n < 65535u ? n : 65535u);
-    k_stencil3_generic<OP><<<grid, block, 0, s>>>(dst, src, w, h, n);
+    GSB_LAUNCH(k_stencil3_generic<OP>, grid, block, 0, s, dst, src, w, h, n);
   }
-  GSB_LAUNCHED(1);
   return 0;
 }
 

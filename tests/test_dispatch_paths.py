@@ -266,6 +266,20 @@ def test_kernel_id_normal_form():
     assert kernel_id("gsb::k_otsu(unsigned char*, unsigned int const*, unsigned int, unsigned int)") == "gsb::k_otsu"
 
 
+def test_launch_policy_lives_in_one_place():
+    """every kernel launch goes through gsb::launch (common.cuh), whose shared-memory opt-in and launch counter are in
+    runtime.cu: so the counter gs_b200_launch_count reports counts each launch once, and no call site opts in by hand"""
+    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "grayskull_b200", "csrc")
+    found = {"<<<": set(), "cudaFuncSetAttribute": set(), "g_launches": set()}
+    for f in sorted(os.listdir(csrc)):
+        with open(os.path.join(csrc, f)) as fh:
+            text = fh.read()
+        for needle, files in found.items():
+            if needle in text:
+                files.add(f)
+    assert found == {"<<<": {"common.cuh"}, "cudaFuncSetAttribute": {"runtime.cu"}, "g_launches": {"runtime.cu"}}, found
+
+
 # ---- GPU -----------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def G():
