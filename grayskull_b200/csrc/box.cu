@@ -27,6 +27,7 @@
 //      inside the image use compile-time constants for count = (2r+1)^2 on a branch-free path,
 //      clipped pixels a 226-entry table.
 // Other radii / widths take the generic kernel (one thread per pixel, any radius).
+#include <limits.h>
 #include <string.h>
 
 #include <type_traits>
@@ -140,9 +141,11 @@ __device__ __forceinline__ uint2 box_finish(const uint32_t (&T)[4], uint2 srcpx,
   uint2 o;
   if (ADAPTIVE) {
     // dst = src > (int)mean - c ? 255 : 0   (reference :244-245), two pixels per 16-bit lane pair:
-    // E = src + (c + 0x7FFF) - mean has bit 15 set exactly when src > mean - c (c clamped to
-    // [-256, 256], beyond which the result saturates anyway); a sign-replicating PRMT turns the
-    // four bit-15s into 0x00 / 0xFF bytes.  q = 0x4B0000mm, so bytes 1 of q are zero.
+    // E = src + (c + 0x7FFF) - mean has bit 15 set exactly when src > mean - c, with c clamped to
+    // [-256, 256]: exact for every c > INT_MIN + 255.  Below that, (int)(mean - (unsigned)c) wraps
+    // negative for large means and the reference writes 255 there; launch_box routes that range to
+    // k_box_wide / k_box_generic, which evaluate the expression literally.  A sign-replicating PRMT
+    // turns the four bit-15s into 0x00 / 0xFF bytes.  q = 0x4B0000mm, so bytes 1 of q are zero.
     const int cc = max(-256, min(256, cparam));
     const uint32_t kc = (uint32_t)(cc + 0x7FFF) * 0x10001u;
     uint32_t e[4];
@@ -999,8 +1002,10 @@ template <bool ADAPTIVE>
 static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, unsigned n, unsigned r,
                       int cparam, cudaStream_t s) {
   if (n == 0) return 0;
+  // the clamped lane compare of k_box_tma / k_box_mid (box_finish) is exact only for c > INT_MIN + 255
+  const bool lane_c_ok = !ADAPTIVE || cparam > INT_MIN + 255;
   CUtensorMap tmap;
-  if (r >= 1 && r <= BX_RMAX && tma_ok(src, w) && tma_ok(dst, w) &&
+  if (lane_c_ok && r >= 1 && r <= BX_RMAX && tma_ok(src, w) && tma_ok(dst, w) &&
       n <= 65535u && make_tmap_u8frames(&tmap, src, w, h, n, BX_PW, BX_TH + 2 * r)) {
     static decltype(&k_box_tma<1, ADAPTIVE>) const box_tma_fn[BX_RMAX] = {
         k_box_tma<1, ADAPTIVE>, k_box_tma<2, ADAPTIVE>, k_box_tma<3, ADAPTIVE>, k_box_tma<4, ADAPTIVE>,
@@ -1028,7 +1033,7 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
     const int fast_ok = (r <= 63 && box_wide_magic((2 * r + 1) * (2 * r + 1), &minv)) ? 1 : 0;
     const bool aligned = w % 8 == 0 && reinterpret_cast<uintptr_t>(src) % 8 == 0 && reinterpret_cast<uintptr_t>(dst) % 8 == 0;
     dim3 grid((strips + 3) / 4, gy, n);
-    if (aligned) {
+    if (aligned && lane_c_ok) {
       // k_box_mid: chunks of 32 rows, so bands are multiples of 32 rows.  Short bands keep the grid many waves deep
       // (3 CTAs of 4 warps per SM); a band re-reads 2r + 1 + 12 rows of its upper neighbour (L2 hits) and spends ~7
       // instructions on each, against ~75 per regular row: the largest of 128 / 64 / 32 rows that still gives

@@ -158,7 +158,8 @@ __global__ void __launch_bounds__(256)
 k_threshold(uint8_t *__restrict__ img, size_t frame_px, const uint8_t *__restrict__ thresh, unsigned scalar,
             int offset) {
   const unsigned f = blockIdx.y;
-  const unsigned t = thresh ? (unsigned)((int)thresh[f] + offset) & 0xFFu : scalar & 0xFFu;
+  // unsigned add: (int)thresh[f] + offset would overflow for offset > INT_MAX - 255; the low byte is the same
+  const unsigned t = thresh ? ((unsigned)thresh[f] + (unsigned)offset) & 0xFFu : scalar & 0xFFu;
   uint8_t *p = img + (size_t)f * frame_px;
   if (VEC) {
     const uint32_t t4 = t * 0x01010101u;

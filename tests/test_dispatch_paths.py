@@ -55,7 +55,10 @@ def _box_rows():
             row("blur", "gsb::k_box_wide<false>", w=256, h=70, r=5, src=4),
             row("blur", "gsb::k_box_wide<false>", w=1080, h=70, r=31, dst=4),
             row("adaptive", "gsb::k_box_wide<true>", w=612, h=70, r=15, c=5),
-            row("adaptive", "gsb::k_box_wide<true>", w=256, h=70, r=3, c=-1, src=4)]
+            row("adaptive", "gsb::k_box_wide<true>", w=256, h=70, r=3, c=-1, src=4),
+            # c <= INT_MIN + 255: the lane compare of k_box_tma / k_box_mid cannot express the wrap, so a TMA geometry
+            # takes k_box_wide
+            row("adaptive", "gsb::k_box_wide<true>", w=272, h=70, r=5, c=-2 ** 31)]
     # r = 0 and r > 120: one thread per pixel
     out += [row("blur", "gsb::k_box_generic<false>", w=200, h=40, r=121),
             row("blur", "gsb::k_box_generic<false>", w=272, h=40, r=0),
@@ -293,6 +296,14 @@ def G():
 def _stream():
     import torch
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+# Have kineto tear CUPTI down at the end of every profiler session, so that each session starts from a fresh CUPTI.
+# Without it, once a process has run some sessions, later ones intermittently deliver no kernel records or only their
+# last kernels (on an H100: 3 of 3 witness probes and 443 sessions of one run of the GPU suite, with every output
+# bit-exact); with it, every session of the same run recorded all its kernels.  Set at import, before the first
+# session of the process: every session of the suite runs through traced().
+os.environ.setdefault("TEARDOWN_CUPTI", "1")
 
 
 def traced(fn):
