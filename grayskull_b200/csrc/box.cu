@@ -284,35 +284,73 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 
 // ---- fused gs_blur(r) -> gs_sobel: the blurred frame never goes to HBM ------------------------
 // gs_b200_blur_sobel_batch(dst, src, r) == gs_blur(tmp, src, r); gs_sobel(dst, tmp) bit for bit (dst's 1-px
-// frame untouched, like gs_sobel), with 1 B/px read + 1 B/px written instead of 4 B/px: the c2 pair of
-// BASELINE.json is HBM-bound, and its intermediate was half of its traffic.  Same walk as k_box_tma: a warp
-// rolls the box sums down its band and gets each blurred row as eight 2^23 + mean floats per lane; instead of
-// packing and storing them, the lane fetches its neighbours' edge quotients by two shuffles and builds gs_sobel's
-// pair words with one PRMT each (pairs.cuh: quot_pairs), keeping the horizontal partials of the previous two
-// blurred rows in registers.  A band of 32 sobel rows needs 34 blurred rows, and sobel needs the blurred columns
-// x-1 / x+8 of the neighbouring lanes.  Lanes 0 and 31 hand on one blurred pixel each, lane 0 its pixel 7 and lane
-// 31 its pixel 0: window_sums<R> gets those two right for every R <= 7, because their windows use only V[4..11]
-// and V[0..7] (lane 0's V[0..3] enter the rolling sum and leave it again exactly, mod 2^32).  So lanes 1..30
-// produce outputs and tiles advance 240 columns, as in k_box_tma.
-// The path is chosen per warp and per lane, not per tile: a warp whose 34 blurred rows all have unclipped row
-// windows takes the unrolled loop, whatever the other warps of its tile do; only the frame's top and bottom bands
-// (and partial bands) take the clipped loop, which reads the division table.  Column clipping never leaves the
-// unrolled loop: each lane divides by its own eight counts (a constant unless it holds column 0 or w-1).  The lanes
-// holding column 0 or w-1 keep dst's byte there by writing the other seven bytes as three stores, so the kernel
-// never reads dst.
-constexpr int BS_UNROLL = 6;                  // rows per unrolled step of the interior band loop (not all 34: the full
-                                              // unroll is 74 KB of SASS and stalls on instruction fetch)
-constexpr int BS_STRIDE = 240;                // output columns per tile (lanes 1..30 x 8 pixels)
-constexpr int BS_TILE_WORDS = BX_PW * (BX_TH + 2 + 2 * BX_RMAX);
-constexpr int BS_SMEM = BS_TILE_WORDS * 4 + 226 * 8 + 16;
+// frame untouched, like gs_sobel), with 1 B/px read + 1 B/px written instead of 4 B/px.  A CTA makes 240 sobel
+// columns x BS_TH rows in two phases with one barrier between them:
+//   A. blur on the tensor cores.  One TMA box loads input bytes [xb, xb + 272) x rows [Y - 8, Y + BS_BROWS + 8),
+//      Y = the tile's first blurred row; outside the image reads as 0, a clipped tap's contribution to the sum.  A
+//      warp walks 16-column strips (blurred columns [c0, c0 + 16), c0 = xb + 8 + 16 s) down the tile:
+//      1. horizontal sums, transposed: H^T = Bh * img with mma.m16n8k32.u8 (A = the constant 0/1 band, 16 output
+//         columns x 32 input columns [c0 - 8, c0 + 24), enough for R <= 8; B = 8 image rows, one LDS.32 per register:
+//         a thread's 4 bytes are consecutive bytes of one row).  H <= 15 * 255 = 3825;
+//      2. H = 256 hi + lo with hi <= 14.  Two such 8-row tiles (a "pair", 16 H rows) hold in each thread exactly the
+//         B fragment of a second MMA over 16 k slots per column (rows 2t, 2t+1 of each tile): four PRMT per column
+//         give its lo and hi operand registers, and the slot order is baked into the constant A of that MMA;
+//      3. vertical sums: S = Bv * H for 16 blurred rows from the 32 H rows of two pairs (A = the constant band over
+//         the permuted slots), once for lo and once for hi.  A step advances 16 rows, so each pair is made once and
+//         used by two steps.  The lo MMA accumulates onto C = 0x4B000000, so IMAD(D_hi, 256, D_lo) is the bit
+//         pattern of the float 2^23 + S (S <= 57375; the MMA sums are exact integers);
+//      4. exact division on the FMA pipe: fma_rd(2^23 + S, m 2^-24, 2^23 - m/2) = 2^23 + floor(S m / 2^24), the same
+//         real value as k_box_tma's fma_rd(S, m 2^-24, 2^23) and rounded once (see div_magic); a strip with a clipped
+//         window anywhere takes each pixel's (inv, k) from the 226-entry table;
+//      5. two quotients of a row are adjacent columns of the MMA's D fragment: one IMAD packs their low bytes, one
+//         STS.U16 stores them to the blurred tile.
+//   B. sobel from the blurred tile, as k_stencil3_tma: each warp walks a 16-row band, each lane 8 columns, with the
+//      previous two rows' partials in registers (pairs.cuh).  The lanes holding column 0 or w-1 keep dst's byte
+//      there by writing the other seven bytes as three stores, so the kernel never reads dst.
+// Blurred pixels outside the image (garbage counts, quotients possibly > 255) come in whole rows or in column pairs
+// (2j, 2j+1) that the packing keeps together, and feed only sobel outputs that are never written.
+constexpr int BS_STRIDE = 240;                 // sobel columns per tile (lanes 0..29 x 8 pixels)
+constexpr int BS_PW = 68;                      // tile pitch in words: 68 = 4 mod 32, conflict-free MMA operand loads
+constexpr int BS_STEPS = 8;                    // 16-row blur steps per tile
+constexpr int BS_WARPS = 8;
+constexpr int BS_THREADS = BS_WARPS * 32;
+constexpr int BS_BROWS = 16 * BS_STEPS;        // blurred rows per tile
+constexpr int BS_TH = BS_BROWS - 2;            // sobel rows per tile
+constexpr int BS_IN_ROWS = BS_BROWS + 16;      // input rows: 8 above and below the blurred rows
+constexpr int BS_STRIPS = 16;                  // 16-column blur strips: blurred columns [xb + 8, xb + 264)
+constexpr int BS_IN_BYTES = BS_PW * 4 * BS_IN_ROWS;
+constexpr int BS_BL_BYTES = BS_PW * 4 * BS_BROWS;
+constexpr int BS_SMEM = BS_IN_BYTES + BS_BL_BYTES + 226 * 8 + 16;
+static_assert(BS_IN_BYTES % 128 == 0, "the blurred tile follows the TMA destination");
+static_assert(BS_TH % 16 == 14, "phase B: the last warp's band is 14 rows");
 
-// division of one row of 8 pixels by the lane's own per-pixel reciprocals inv[i] (see div_magic)
-__device__ __forceinline__ void box_quot_lanes(const uint32_t (&T)[4], const float (&inv)[8], uint32_t (&q)[8]) {
-#pragma unroll
-  for (int p = 0; p < 4; p++) {
-    q[2 * p] = div_lo(T[p], inv[2 * p]);
-    q[2 * p + 1] = div_hi(T[p], inv[2 * p + 1]);
+// div_magic of every count 1..225 as a compile-time table: a tile with clipped windows copies it to shared memory
+// (the integer division of div_magic would put I2F / MUFU work in the kernel's prologue)
+struct DivMagicTable {
+  float2 e[226];
+};
+constexpr DivMagicTable make_div_magic_table() {
+  DivMagicTable t{};
+  for (unsigned c = 1; c < 226; c++) {
+    const unsigned m = (16777216u + c - 1u) / c;
+    t.e[c].x = (float)m * 5.9604644775390625e-08f;
+    t.e[c].y = 8388608.0f - 0.5f * (float)m;
   }
+  return t;
+}
+__constant__ DivMagicTable c_div_magic = make_div_magic_table();
+
+// D (+)= A (16x32 u8, row) * B (32x8 u8, col), s32 accumulators
+__device__ __forceinline__ void mma_u8(uint32_t (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1, uint32_t c) {
+  asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%10, %10, %10, %10};"
+      : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1), "r"(c));
+}
+__device__ __forceinline__ uint32_t imad256(uint32_t hi, uint32_t lo) {   // hi * 256 + lo on the FMA pipe
+  uint32_t d;
+  asm("mad.lo.u32 %0, %1, 256, %2;" : "=r"(d) : "r"(hi), "r"(lo));
+  return d;
 }
 
 // the 8 output bytes of a lane whose first byte is image column 0 (left) or whose last is column w-1 (!left): the
@@ -330,149 +368,190 @@ __device__ __forceinline__ void st_cs_7of8(uint8_t *p, uint2 v, bool left) {
 }
 
 template <int R>
-__global__ void __launch_bounds__(BX_THREADS)
+__global__ void __launch_bounds__(BS_THREADS, 3)
 k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, unsigned w, unsigned h) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  uint32_t *tile = reinterpret_cast<uint32_t *>(smem_raw);
-  float2 *magic = reinterpret_cast<float2 *>(smem_raw + BS_TILE_WORDS * 4);
-  uint64_t &bar = *reinterpret_cast<uint64_t *>(smem_raw + BS_TILE_WORDS * 4 + 226 * 8);
-  constexpr int ROWS = BX_TH + 2 + 2 * R;
+  const uint32_t *in = reinterpret_cast<const uint32_t *>(smem_raw);          // input row i = image row Y - 8 + i
+  unsigned char *bl = smem_raw + BS_IN_BYTES;                                 // blurred row i = image row Y + i
+  float2 *magic = reinterpret_cast<float2 *>(smem_raw + BS_IN_BYTES + BS_BL_BYTES);
+  uint64_t &bar = *reinterpret_cast<uint64_t *>(smem_raw + BS_IN_BYTES + BS_BL_BYTES + 226 * 8);
   constexpr int FULL = 2 * R + 1;
+  constexpr unsigned FM = (16777216u + FULL * FULL - 1u) / (FULL * FULL);
+  constexpr float FINV = (float)FM * 5.9604644775390625e-08f, FK = 8388608.0f - 0.5f * (float)FM;   // div_magic
 
   const unsigned frame = blockIdx.z;
   const int xb = (int)blockIdx.x * BS_STRIDE - 16;   // image column of tile byte 0 (16-B aligned)
-  const int y0 = (int)blockIdx.y * BX_TH;            // first sobel row of the tile
+  const int y0 = (int)blockIdx.y * BS_TH;            // first sobel row of the tile
+  const int Y = y0 - 1;                              // first blurred row
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
     mbar_fence_init();
-    mbar_expect_tx(&bar, BX_PW * 4 * ROWS);
-    tma_load_3d(tile, &tmap, xb / 4, y0 - 1 - R, frame, &bar);
+    mbar_expect_tx(&bar, BS_IN_BYTES);
+    tma_load_3d(smem_raw, &tmap, xb / 4, Y - 8, frame, &bar);
   }
-  // the clipped-count division table, only where some warp's band has row-clipped windows (the tile holds the
-  // frame's first or last rows); it is built while the tile is in flight
-  if (y0 - 1 - R < 0 || y0 + BX_TH + R > (int)h - 1) {
-    for (unsigned c = threadIdx.x + 1; c < 226; c += BX_THREADS) {
-      const DivMagic d = div_magic(c);
-      magic[c] = make_float2(d.inv, d.k);
-    }
+  // the clipped-count division table, only in tiles with a clipped blurred pixel; built while the tile is in flight
+  if (Y - R < 0 || Y + BS_BROWS - 1 + R > (int)h - 1 || xb + 8 - R < 0 || xb + 8 + 16 * BS_STRIPS - 1 + R > (int)w - 1) {
+    for (unsigned c = threadIdx.x + 1; c < 226; c += BS_THREADS) magic[c] = c_div_magic.e[c];
   }
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int x = xb + 8 * lane;
-  const int yb = y0 + warp * BX_BH;            // first sobel row of this warp's band; blurred rows yb-1 .. yb+BH
-  // every row window of the band's blurred rows is unclipped: the unrolled loop.  Warp-uniform; the vote tells the
-  // compiler so, and the loop's shuffles then need no convergence check
-  const bool rows_full = __all_sync(0xFFFFFFFFu, yb - 1 - R >= 0 && yb + BX_BH + R <= (int)h - 1);
-  // lanes 0 and 31 need the right counts for the pixel they hand on; the first tile's lane 1 sits at column -8, so
-  // its outputs start at lane 2
-  const bool blur_lane = x >= 0 && x < (int)w;
-  const bool out_lane = lane >= 1 && lane <= 30 && x >= 0 && x < (int)w;
-  const uint32_t *in = tile + (warp * BX_BH) * BX_PW + 2 * lane;   // tile row of image row yb - 1 - R
-  uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
-  // the quotients of lanes outside the image are wrong (made-up counts) and may exceed 255: an output lane takes
-  // only the low byte of its neighbours' edge quotients (quot_pairs), which then feeds only pixel x (left neighbour
-  // outside: x = 0) or x+7 (right neighbour outside: x+7 = w-1), and both keep dst's bytes
-  int cw[8];
+  const int g = lane >> 2, t = lane & 3;             // MMA fragment coordinates
+  // the constant A operands: ah = horizontal band (row = output column c, k = input column c0 - 8 + k), av = vertical
+  // band (row = blurred row y of the step, k = H row slot; slot 4t'+i of a pair holds tile i>>1, row 2t' + (i&1))
+  uint32_t ah[4], av[4];
 #pragma unroll
-  for (int j = 0; j < 8; j++) cw[j] = blur_lane ? min(x + j + R, (int)w - 1) - max(x + j - R, 0) + 1 : 1;
-  // the unrolled loop's per-pixel reciprocals of count = cw * (2R+1): the same values as the table's, a constant
-  // except in the lanes of columns 0 and w-8 (R <= 7 < 8), the only ones with clipped column windows
-  constexpr float FINV = (float)((16777216u + FULL * FULL - 1u) / (FULL * FULL)) * 5.9604644775390625e-08f;
-  float inv[8];
+  for (int j = 0; j < 4; j++) {
+    const int row = g + 8 * (j & 1), kb = 16 * (j >> 1) + 4 * t;
+    uint32_t a = 0, v = 0;
 #pragma unroll
-  for (int j = 0; j < 8; j++) inv[j] = FINV;
-  if (blur_lane && (x - R < 0 || x + 7 + R > (int)w - 1)) {
-#pragma unroll
-    for (int j = 0; j < 8; j++) inv[j] = div_magic(cw[j] * FULL).inv;
+    for (int i = 0; i < 4; i++) {
+      const int k = kb + i;
+      const int hrow = (k >> 4) * 16 + ((k >> 1) & 1) * 8 + 2 * ((k >> 2) & 3) + (k & 1);   // relative to y - 8
+      a |= (uint32_t)(abs(k - 8 - row) <= R) << (8 * i);
+      v |= (uint32_t)(abs(hrow - 8 - row) <= R) << (8 * i);
+    }
+    ah[j] = a, av[j] = v;
   }
-  const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
+
+  // built once per thread (the compiler would rebuild them per strip)
+#pragma unroll
+  for (int j = 0; j < 4; j++) asm("" : "+r"(ah[j]), "+r"(av[j]));
+  // interior division constants, in registers (FFMA takes one immediate)
+  float finv = FINV, fk = FK;
+  asm("" : "+f"(finv), "+f"(fk));
+  const bool rows_full = Y - R >= 0 && Y + BS_BROWS - 1 + R <= (int)h - 1;
 
   mbar_wait(&bar, 0);
-  if (yb >= (int)h - 1) return;                // warp-uniform: no sobel row of this band is written
 
-  uint32_t S[4] = {0, 0, 0, 0};
+  // ---- phase A: blurred tile
+  for (int s = warp; s < BS_STRIPS; s += BS_WARPS) {
+    const int c0 = xb + 8 + 16 * s;                  // image column of the strip's first blurred column
+    if (c0 >= (int)w) break;                         // warp-uniform
+    const uint32_t *ip = in + g * BS_PW + 4 * s + t;
+    unsigned char *bp = bl + g * (BS_PW * 4) + 16 * s + 2 * t;
+    const bool cols_full = c0 - R >= 0 && c0 + 15 + R <= (int)w - 1;
+    // clipped column counts of the thread's four columns c0 + 8 hh + 2t + e
+    int cw[4];
 #pragma unroll
-  for (int i = 0; i < 2 * R; i++) {
-    uint32_t e[4];
-    unpack_pairs(*reinterpret_cast<const uint2 *>(in + i * BX_PW), e);
+    for (int j = 0; j < 4; j++) {
+      const int c = c0 + 8 * (j >> 1) + 2 * t + (j & 1);
+      cw[j] = max(min(c + R, (int)w - 1) - max(c - R, 0) + 1, 1);
+    }
+    // lo / hi operands of a pair of 8-row H tiles (input rows 16 p .. 16 p + 15), both column halves
+    auto make_pair = [&](int p, uint32_t (&o)[4]) {
+      uint32_t P[4], Q[4];
+      const uint32_t *r0 = ip + 16 * p * BS_PW, *r1 = r0 + 8 * BS_PW;
+      mma_u8(P, ah, r0[0], r0[4], 0u);
+      mma_u8(Q, ah, r1[0], r1[4], 0u);
 #pragma unroll
-    for (int k = 0; k < 4; k++) S[k] += e[k];
+      for (int hh = 0; hh < 2; hh++) {
+        const uint32_t x = prmt(P[2 * hh], P[2 * hh + 1], 0x5140), y = prmt(Q[2 * hh], Q[2 * hh + 1], 0x5140);
+        o[2 * hh] = prmt(x, y, 0x5410);        // lo bytes
+        o[2 * hh + 1] = prmt(x, y, 0x7632);    // hi bytes
+      }
+    };
+    // pairs u and u+1 in registers pa / pb: pair u + 1 overwrites pair u - 1, so the MMA's B operand is (pa, pb) at
+    // every step, and odd steps take the band with its two k halves swapped (slots 0..15 = pair u + 1)
+    uint32_t pa[4], pb[4];
+    make_pair(0, pa);
+    auto walk = [&](auto full_tag) {
+      constexpr bool FULLW = decltype(full_tag)::value;
+#pragma unroll
+      for (int u = 0; u < BS_STEPS; u++) {
+        const int yu = Y + 16 * u;
+        if (yu >= (int)h) break;                     // warp-uniform: blurred rows below the image are never used
+        make_pair(u + 1, pb);
+        int ch[2] = {FULL, FULL};
+        if (!FULLW) {
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int y = yu + g + 8 * e;
+            ch[e] = max(min(y + R, (int)h - 1) - max(y - R, 0) + 1, 1);
+          }
+        }
+#pragma unroll
+        for (int hh = 0; hh < 2; hh++) {
+          uint32_t dl[4], dh[4];
+          mma_u8(dl, av, pa[2 * hh], pb[2 * hh], 0x4B000000u);
+          mma_u8(dh, av, pa[2 * hh + 1], pb[2 * hh + 1], 0u);
+          uint32_t q[4];
+#pragma unroll
+          for (int j = 0; j < 4; j++) {             // D element j: row g + 8 (j >> 1), column 8 hh + 2t + (j & 1)
+            float inv = finv, k = fk;
+            if (!FULLW) {
+              const float2 m = magic[cw[2 * hh + (j & 1)] * ch[j >> 1]];
+              inv = m.x, k = m.y;
+            }
+            q[j] = __float_as_uint(__fmaf_rd(__uint_as_float(imad256(dh[j], dl[j])), inv, k));
+          }
+          unsigned char *o = bp + 16 * u * (BS_PW * 4) + 8 * hh;
+          *reinterpret_cast<uint16_t *>(o) = (uint16_t)imad256(q[1], q[0]);
+          *reinterpret_cast<uint16_t *>(o + 8 * (BS_PW * 4)) = (uint16_t)imad256(q[3], q[2]);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; j++) pa[j] = pb[j];
+      }
+    };
+    // windows clipped anywhere in the strip: per-pixel counts from the table
+    if (cols_full && rows_full) walk(std::true_type{});
+    else walk(std::false_type{});
   }
-  uint32_t L[4] = {0, 0, 0, 0};
+  __syncthreads();
 
-  // blurred row j of the band (image row yb - 1 + j) as eight 2^23 + mean floats
-  auto blur_row = [&](int j, auto interior_tag, uint32_t (&q)[8]) {
-    constexpr bool INT = decltype(interior_tag)::value;
-    uint32_t e[4];
-    unpack_pairs(*reinterpret_cast<const uint2 *>(in + (j + 2 * R) * BX_PW), e);
-#pragma unroll
-    for (int k = 0; k < 4; k++) S[k] = S[k] + e[k] - L[k];
-    unpack_pairs(*reinterpret_cast<const uint2 *>(in + j * BX_PW), L);
-    uint32_t V[12], T[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-      V[4 + k] = S[k];
-      V[k] = (R == 7 || k > 0) ? __shfl_up_sync(0xFFFFFFFFu, S[k], 1) : 0u;
-      V[8 + k] = (R == 7 || k < 3) ? __shfl_down_sync(0xFFFFFFFFu, S[k], 1) : 0u;
-    }
-    window_sums<R>(V, T);
-    if (INT) {
-      box_quot_lanes(T, inv, q);
-    } else {
-      const int y = yb - 1 + j;
-      const int ch = max(min(y + R, (int)h - 1) - max(y - R, 0) + 1, 1);   // rows outside the image are never used
-      box_quot<R, false>(T, cw, ch, magic, q);
-    }
+  // ---- phase B: sobel rows y0 + 16 warp .. + nb - 1 from blurred rows one above to one below
+  const int r0 = 16 * warp, nb = min(16, BS_TH - r0);
+  const int x = xb + 16 + 8 * lane;
+  const int yb = y0 + r0;
+  const bool live = lane < 30 && x < (int)w;
+  const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
+  // a warp with a lane on column 0 or w-1 walks its own copy, so that the others keep the single 64-bit store
+  const bool edge_warp = __any_sync(0xFFFFFFFFu, live && (edge_l || edge_r));
+  if (!live || yb > (int)h - 2) return;
+  const uint32_t *base = reinterpret_cast<const uint32_t *>(bl) + r0 * BS_PW + 2 * lane + 1;   // blurred bytes x-4 ..
+  auto load_row = [&](int r) -> SobelRow {
+    const uint32_t *p = base + r * BS_PW;
+    const uint2 wm = *reinterpret_cast<const uint2 *>(p + 1);
+    return sobel_row(split_pairs(p[0], wm.x, wm.y, p[3]));
   };
-
-  // the lanes of columns 0 and w-1 keep dst's byte there; all three stores are predicated, no lane branches
-  const bool st_all = out_lane && !edge_l && !edge_r, st_l = out_lane && edge_l, st_r = out_lane && edge_r;
-  const bool edge_warp = __any_sync(0xFFFFFFFFu, st_l || st_r);
-  auto store = [&](uint2 so) {
-    if (st_all) st_cs_u2(outp, so);
-    if (st_l) st_cs_7of8(outp, so, true);
-    if (st_r) st_cs_7of8(outp, so, false);
-  };
-  SobelRow ra, rb;
-  auto sobel_step = [&](int j, const uint32_t (&q)[8], bool write_row, auto interior_tag, auto edge_tag) {
-    const uint32_t qm1 = __shfl_up_sync(0xFFFFFFFFu, q[7], 1);    // blurred pixel x-1
-    const uint32_t q8 = __shfl_down_sync(0xFFFFFFFFu, q[0], 1);   // blurred pixel x+8
-    const SobelRow rc = sobel_row(quot_pairs(qm1, q, q8));
-    if (j >= 2) {
-      if (decltype(interior_tag)::value) {
-        const uint2 so = sobel_out(ra, rb, rc);  // outside the branch, so that the store is predicated
-        if (decltype(edge_tag)::value) store(so);
-        else if (out_lane) st_cs_u2(outp, so);
-      } else if (write_row) {
-        store(sobel_out(ra, rb, rc));
+  uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
+  SobelRow ra = load_row(0), rb = load_row(1);
+  auto walk_full = [&](auto edge_tag) {
+#pragma unroll
+    for (int i = 0; i < 16; i++) {
+      if (i >= BS_TH % 16 && i >= nb) break;
+      const SobelRow rc = load_row(i + 2);
+      const uint2 so = sobel_out(ra, rb, rc);
+      if (!decltype(edge_tag)::value) {
+        st_cs_u2(outp, so);
+      } else {                                       // predicated, no lane branches
+        if (!edge_l && !edge_r) st_cs_u2(outp, so);
+        if (edge_l) st_cs_7of8(outp, so, true);
+        if (edge_r) st_cs_7of8(outp, so, false);
       }
       outp += w;
-    }
-    ra = rb;
-    rb = rc;
-  };
-
-  // unrolled walk; a warp with a lane on column 0 or w-1 gets its own copy, so that the others store as before
-  auto walk_rows_full = [&](auto edge_tag) {
-#pragma unroll BS_UNROLL
-    for (int j = 0; j < BX_BH + 2; j++) {
-      uint32_t q[8];
-      blur_row(j, std::true_type{}, q);
-      sobel_step(j, q, true, std::true_type{}, edge_tag);
+      ra = rb;
+      rb = rc;
     }
   };
-  if (rows_full) {
-    if (edge_warp) walk_rows_full(std::true_type{});
-    else walk_rows_full(std::false_type{});
+  if (yb >= 1 && yb + nb - 1 <= (int)h - 2) {
+    if (edge_warp) walk_full(std::true_type{});
+    else walk_full(std::false_type{});
   } else {
 #pragma unroll 1
-    for (int j = 0; j < BX_BH + 2; j++) {
-      const int ys = yb + j - 2;                 // the sobel row completed by blurred row j
-      if (ys > (int)h - 2) break;                // warp-uniform
-      uint32_t q[8];
-      blur_row(j, std::false_type{}, q);
-      sobel_step(j, q, ys >= 1, std::false_type{}, std::true_type{});
+    for (int i = 0; i < nb; i++) {
+      const int y = yb + i;
+      if (y > (int)h - 2) break;
+      const SobelRow rc = load_row(i + 2);
+      if (y >= 1) {
+        const uint2 so = sobel_out(ra, rb, rc);
+        if (edge_l) st_cs_7of8(outp, so, true);
+        else if (edge_r) st_cs_7of8(outp, so, false);
+        else st_cs_u2(outp, so);
+      }
+      outp += w;
+      ra = rb;
+      rb = rc;
     }
   }
 }
@@ -1073,13 +1152,13 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
   if (n == 0 || w < 3 || h < 3) return 0;    // gs_sobel writes nothing below 3x3 (reference :308-309)
   CUtensorMap tmap;
   if (radius >= 1 && radius <= gsb::BX_RMAX && gsb::tma_ok(src, w) && gsb::tma_ok(dst, w) && n <= 65535u &&
-      gsb::make_tmap_u8frames(&tmap, src, w, h, n, gsb::BX_PW, gsb::BX_TH + 2 + 2 * radius)) {
+      gsb::make_tmap_u8frames(&tmap, src, w, h, n, gsb::BS_PW, gsb::BS_IN_ROWS)) {
     static decltype(&gsb::k_blur_sobel_tma<1>) const blur_sobel_fn[gsb::BX_RMAX] = {
         gsb::k_blur_sobel_tma<1>, gsb::k_blur_sobel_tma<2>, gsb::k_blur_sobel_tma<3>, gsb::k_blur_sobel_tma<4>,
         gsb::k_blur_sobel_tma<5>, gsb::k_blur_sobel_tma<6>, gsb::k_blur_sobel_tma<7>};
-    const unsigned tiles_x = (w + 8 + gsb::BS_STRIDE - 1) / gsb::BS_STRIDE, tiles_y = (h + gsb::BX_TH - 1) / gsb::BX_TH;
+    const unsigned tiles_x = (w + gsb::BS_STRIDE - 1) / gsb::BS_STRIDE, tiles_y = (h + gsb::BS_TH - 1) / gsb::BS_TH;
     GSB_ASSERT(tiles_y <= 65535u);
-    GSB_LAUNCH(blur_sobel_fn[radius - 1], dim3(tiles_x, tiles_y, n), gsb::BX_THREADS, gsb::BS_SMEM, s, tmap, dst, w, h);
+    GSB_LAUNCH(blur_sobel_fn[radius - 1], dim3(tiles_x, tiles_y, n), gsb::BS_THREADS, gsb::BS_SMEM, s, tmap, dst, w, h);
     return 0;
   }
   // other radii / ragged widths: the two per-op kernels through a scratch frame batch (same result, 4 B/px)

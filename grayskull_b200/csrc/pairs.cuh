@@ -26,23 +26,6 @@ __device__ __forceinline__ Pairs split_pairs(uint32_t wl, uint32_t w0, uint32_t 
   return p;
 }
 
-// the same pair words from per-pixel words whose low byte is the pixel and whose byte 1 is zero (the box kernels'
-// quotient floats 2^23 + b = 0x4B0000bb): q[k] = pixel x+k, qm1 = pixel x-1, q8 = pixel x+8.  One PRMT per pair
-// word.  Only the low byte of the neighbours' qm1 / q8 is taken (the zero bytes come from q), so a neighbour lane
-// outside the image, whose quotient may exceed 255, changes only the 16-bit lane of pixel x-1 / x+8 and no other.
-__device__ __forceinline__ Pairs quot_pairs(uint32_t qm1, const uint32_t (&q)[8], uint32_t q8) {
-  Pairs p;
-  p.m1 = prmt(qm1, q[1], 0x5450);
-  p.p0 = prmt(q[0], q[2], 0x5410);
-  p.p1 = prmt(q[1], q[3], 0x5410);
-  p.p2 = prmt(q[2], q[4], 0x5410);
-  p.p3 = prmt(q[3], q[5], 0x5410);
-  p.p4 = prmt(q[4], q[6], 0x5410);
-  p.p5 = prmt(q[5], q[7], 0x5410);
-  p.p6 = prmt(q[6], q8, 0x1410);
-  return p;
-}
-
 __device__ __forceinline__ __half2 as_h2(uint32_t v) { return *reinterpret_cast<__half2 *>(&v); }
 __device__ __forceinline__ uint32_t as_u32(__half2 v) { return *reinterpret_cast<uint32_t *>(&v); }
 
