@@ -1,7 +1,9 @@
-"""ctypes loaders shared by the tests: the oracle restatement, the real reference build
-(oracle/_ref, when present) and synthetic-input generators.  TEST INFRASTRUCTURE only."""
+"""ctypes loaders shared by the tests: the oracle restatement and numpy wrappers of its calls, the real reference build
+(oracle/_ref, when present), synthetic-input generators and the built library's SASS.  TEST INFRASTRUCTURE only."""
 import ctypes as C
 import os
+import re
+import shutil
 import subprocess
 
 import numpy as np
@@ -115,6 +117,41 @@ def oracle():
                                        C.c_uint, C.c_float, C.c_float, C.c_float, C.c_int]
         _cache["o"] = lib
     return _cache["o"]
+
+
+# ---- oracle calls on numpy arrays (O = oracle()) ---------------------------------------------------------------------
+def o_blur(O, a, r):
+    d = np.empty_like(a); O.gso_blur(ptr(d), ptr(a), a.shape[1], a.shape[0], r); return d
+def o_adaptive(O, a, r, c):
+    d = np.empty_like(a); O.gso_adaptive_threshold(ptr(d), ptr(a), a.shape[1], a.shape[0], r, c); return d
+def o_morph(O, a, dil):
+    d = np.empty_like(a); O.gso_morph(ptr(d), ptr(a), a.shape[1], a.shape[0], dil); return d
+def o_sobel(O, a, fill=0):
+    """gso_sobel into an array of `fill`: its 1-px frame keeps `fill` (an array: a copy of it)"""
+    d = np.array(np.broadcast_to(fill, a.shape), np.uint8)
+    O.gso_sobel(ptr(d), ptr(a), a.shape[1], a.shape[0]); return d
+def o_resize(O, a, dw, dh):
+    d = np.empty((dh, dw), np.uint8); O.gso_resize(ptr(d), dw, dh, ptr(a), a.shape[1], a.shape[0]); return d
+def o_down(O, a):
+    d = np.empty((a.shape[0] // 2, a.shape[1] // 2), np.uint8); O.gso_downsample(ptr(d), ptr(a), a.shape[1], a.shape[0]); return d
+def o_integral(O, a):
+    ii = np.empty(a.shape, np.uint32); O.gso_integral(ptr(a), a.shape[1], a.shape[0], ptr(ii)); return ii
+def o_fast(O, a, sm, nkps, t):
+    k = np.zeros(nkps, KP_DTYPE)
+    n = O.gso_fast(ptr(a), a.shape[1], a.shape[0], ptr(sm), sm.shape[1], sm.shape[0], ptr(k), nkps, t)
+    return k[:n]
+def o_orb(O, a, sm, nkps, t):
+    k = np.zeros(nkps, KP_DTYPE)
+    n = O.gso_orb_extract(ptr(a), a.shape[1], a.shape[0], ptr(k), nkps, t, ptr(sm))
+    return k[:n]
+def o_detect(O, cas, ii, max_rects, sf, mn, mx, step):
+    r = np.zeros(max(max_rects, 1), RECT_DTYPE)
+    n = O.gso_lbp_detect(cas.ptr, ptr(ii), ii.shape[1], ii.shape[0], ptr(r), max_rects, sf, mn, mx, step)
+    return r[:n]
+def o_match(O, k1, k2, mm, md):
+    m = np.zeros(max(1, min(mm, len(k1))), MATCH_DTYPE)          # at most one match per query
+    n = O.gso_match_orb(ptr(k1), len(k1), ptr(k2 if len(k2) else np.zeros(1, KP_DTYPE)), len(k2), ptr(m), mm, md)
+    return m[:n]
 
 
 def have_ref():
@@ -340,3 +377,75 @@ def oracle_chain(cascade_ptr, frame, **params):
     nr = O.gso_lbp_detect(cascade_ptr, L.ptr(t), w, h, L.ptr(r), p["max_rects"], p["scale_factor"], p["min_scale"],
                           p["max_scale"], p["step"])
     return {"sobel": s, "kps": k[:nk], "rects": r[:nr]}
+
+
+def otsu_images(rng):
+    """bimodal, flat, two-level, dark-heavy, noise and near-tie images: exercises wb == 0 skips, the wf == 0
+    break and fp32 ties in varBetween"""
+    out = []
+    for (w, h) in ((3, 3), (64, 48), (257, 31), (640, 480), (1, 1), (5, 1)):
+        out.append(rng.integers(0, 256, (h, w), dtype=np.uint8))
+        a = np.where(rng.random((h, w)) < 0.3, rng.normal(60, 12, (h, w)), rng.normal(190, 20, (h, w)))
+        out.append(np.clip(a, 0, 255).astype(np.uint8))
+        out.append(np.full((h, w), int(rng.integers(0, 256)), np.uint8))
+        b = np.full((h, w), 10, np.uint8); b.flat[:: max(1, (w * h) // 7)] = 250
+        out.append(b)
+        out.append((rng.integers(0, 2, (h, w)) * 255).astype(np.uint8))
+        out.append(rng.integers(100, 104, (h, w), dtype=np.uint8))
+    out.append(natural_like(1920, 1080, 3))
+    return out
+
+
+# ---- kernel names and the built library's SASS -----------------------------------------------------------------------
+def kernel_id(name):
+    """a demangled kernel name (kineto's 'void gsb::k_box_mid<1, false>(CUtensorMap_st, ...)' or cu++filt's
+    'void gsb::k_box_mid<(int)1, (bool)0>(...)') -> 'gsb::k_box_mid<1,false>'"""
+    s = name.strip()
+    if s.startswith("void "):
+        s = s[5:]
+    depth = 0
+    for i, ch in enumerate(s):
+        depth += ch == "<"
+        depth -= ch == ">"
+        if ch == "(" and depth == 0:
+            s = s[:i]
+            break
+    s = s.replace("(bool)0", "false").replace("(bool)1", "true")
+    s = re.sub(r"\((?:unsigned )?int\)(-?\d+)", r"\1", s)
+    s = re.sub(r"\b(\d+)u\b", r"\1", s)
+    return s.replace(" ", "")
+
+
+def cuda_tool(name):
+    """a CUDA toolkit binary from PATH, else from /usr/local/cuda/bin; None when neither has it"""
+    tool = shutil.which(name) or os.path.join("/usr/local/cuda/bin", name)
+    return tool if os.path.exists(tool) else None
+
+
+def demangle(names):
+    """cu++filt over mangled names (returned as they are without the tool)"""
+    tool = cuda_tool("cu++filt")
+    if not names or tool is None:
+        return list(names)
+    out = subprocess.run([tool], input="\n".join(names) + "\n", capture_output=True, text=True, check=True).stdout
+    return out.splitlines()
+
+
+def sass_functions():
+    """{kernel_id: SASS} of every function in the built library, from one `cuobjdump -sass` per process.  Each SASS
+    starts with the 'code for sm_XX' line of the cubin that holds it.  Skips the calling test without cuobjdump."""
+    if "sass" not in _cache:
+        import pytest
+        from grayskull_b200 import _lib
+        tool = cuda_tool("cuobjdump")
+        if tool is None:
+            pytest.skip("cuobjdump not found")
+        listing = subprocess.run([tool, "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+        funcs = {}
+        for cubin in re.split(r"^\s*(?=code for sm_\w+\s*$)", listing, flags=re.M)[1:]:
+            arch, *parts = re.split(r"^\s*Function : (\S+)\s*$", cubin, flags=re.M)
+            arch = arch.strip().splitlines()[0]
+            for name, body in zip(demangle(parts[0::2]), parts[1::2]):
+                funcs[kernel_id(name)] = arch + "\n" + body
+        _cache["sass"] = funcs
+    return _cache["sass"]

@@ -14,16 +14,14 @@ dispatch geometry per row (op, sizes, a byte offset for each base) and the kerne
   * CPU (census): every kernel in the built library's SASS is named by a row or sits in ALLOWED with its reason, so
     a kernel added without a row fails without a GPU.
 """
-import ctypes as C
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import _libs as L
+from _gpu import O, Region, frames, kernel_id, lib, stream, traced, witness, witnessed  # noqa: F401
 
 
 def row(op, kernels, **p):
@@ -204,38 +202,6 @@ def row_id(op, p):
     return "-".join([op] + ["%s%s" % (k, v) for k, v in p.items() if k != "n"] + ["n%d" % p["n"]])
 
 
-def kernel_id(name):
-    """a demangled kernel name (kineto's 'void gsb::k_box_mid<1, false>(CUtensorMap_st, ...)' or cu++filt's
-    'void gsb::k_box_mid<(int)1, (bool)0>(...)') -> 'gsb::k_box_mid<1,false>'"""
-    s = name.strip()
-    if s.startswith("void "):
-        s = s[5:]
-    depth = 0
-    for i, ch in enumerate(s):
-        depth += ch == "<"
-        depth -= ch == ">"
-        if ch == "(" and depth == 0:
-            s = s[:i]
-            break
-    s = s.replace("(bool)0", "false").replace("(bool)1", "true")
-    s = re.sub(r"\((?:unsigned )?int\)(-?\d+)", r"\1", s)
-    s = re.sub(r"\b(\d+)u\b", r"\1", s)
-    return s.replace(" ", "")
-
-
-def _cuda_tool(name):
-    tool = shutil.which(name) or os.path.join("/usr/local/cuda/bin", name)
-    return tool if os.path.exists(tool) else None
-
-
-def _demangle(names):
-    tool = _cuda_tool("cu++filt")
-    if not names or tool is None:
-        return list(names)
-    out = subprocess.run([tool], input="\n".join(names) + "\n", capture_output=True, text=True, check=True).stdout
-    return out.splitlines()
-
-
 # ---- CPU: the census -----------------------------------------------------------------------------------------------
 def test_rows_are_unique_and_well_formed():
     ids = [row_id(op, p) for op, _, p in ROWS]
@@ -247,13 +213,7 @@ def test_rows_are_unique_and_well_formed():
 
 
 def test_every_kernel_has_a_row():
-    from grayskull_b200 import _lib
-    tool = _cuda_tool("cuobjdump")
-    if tool is None:
-        pytest.skip("cuobjdump not found")
-    sass = subprocess.run([tool, "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    mangled = re.findall(r"^\s*Function : (\S+)\s*$", sass, flags=re.M)
-    built = {kernel_id(n) for n in _demangle(mangled)}
+    built = set(L.sass_functions())
     assert len(built) > 50, sorted(built)
     table = {kernel_id(k) for _, kernels, _ in ROWS for k in kernels}
     orphans = sorted(k for k in built if k not in table and not any(re.fullmatch(a, k) for a in ALLOWED))
@@ -284,91 +244,6 @@ def test_launch_policy_lives_in_one_place():
 
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def G():
-    import torch
-    import grayskull_b200 as g
-    assert torch.cuda.is_available()
-    g.lib().gs_b200_set_device(0)
-    return g.lib()
-
-
-def _stream():
-    import torch
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-# Have kineto tear CUPTI down at the end of every profiler session, so that each session starts from a fresh CUPTI.
-# Without it, once a process has run some sessions, later ones intermittently deliver no kernel records or only their
-# last kernels (on an H100: 3 of 3 witness probes and 443 sessions of one run of the GPU suite, with every output
-# bit-exact); with it, every session of the same run recorded all its kernels.  Set at import, before the first
-# session of the process: every session of the suite runs through traced().
-os.environ.setdefault("TEARDOWN_CUPTI", "1")
-
-
-def traced(fn):
-    """run fn (a C call returning its status) under torch.profiler with CUDA activity -> (status, launched kernels)"""
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        rc = fn()
-        torch.cuda.synchronize()
-    names = {e.name for e in prof.events() if "k_" in e.name}
-    mangled = sorted(nm for nm in names if nm.startswith("_Z"))
-    names = (names - set(mangled)) | set(_demangle(mangled))
-    return rc, {kernel_id(nm) for nm in names if "gsb::" in nm}
-
-
-@pytest.fixture(scope="module")
-def witness(G):
-    """whether kineto sees the library's launches at all: one probe launch"""
-    import torch
-    src = torch.zeros((1, 40, 272), dtype=torch.uint8, device="cuda")
-    out = torch.empty_like(src)
-    rc, seen = traced(lambda: G.gs_b200_blur_batch(out.data_ptr(), src.data_ptr(), 272, 40, 1, 5, _stream()))
-    assert rc == 0
-    print("\nwitness probe: %s" % (sorted(seen) or "no kernel events recorded"))
-    return bool(seen)
-
-
-class Region:
-    """`nbytes` at byte `off` of a 256-byte aligned device allocation of nbytes + 32 bytes.  Everything starts as a
-    seeded byte pattern (then `data`, if given, in the view); read() checks that the bytes outside the view kept it."""
-
-    def __init__(self, nbytes, off=0, data=None, seed=0):
-        import torch
-        self.off, self.nbytes = off, nbytes
-        self.host = np.random.default_rng(seed * 7919 + nbytes + off).integers(0, 256, nbytes + 32, dtype=np.uint8)
-        if data is not None:
-            b = np.frombuffer(np.ascontiguousarray(data).tobytes(), np.uint8)
-            assert b.size == nbytes
-            self.host[off:off + nbytes] = b
-        self.t = torch.from_numpy(self.host.copy()).cuda()
-        assert self.t.data_ptr() % 256 == 0
-        self.ptr = self.t.data_ptr() + off
-
-    def before(self):
-        return self.host[self.off:self.off + self.nbytes].copy()
-
-    def read(self, what):
-        got = self.t.cpu().numpy()
-        o, e = self.off, self.off + self.nbytes
-        assert np.array_equal(got[:o], self.host[:o]) and np.array_equal(got[e:], self.host[e:]), \
-            "%s: bytes outside the view changed" % what
-        return got[o:e].copy()
-
-
-def frames(w, h, n, seed):
-    """random, natural_like and saturated (255) frames in turn"""
-    rng = np.random.default_rng(seed)
-    out = []
-    for i in range(n):
-        out.append([rng.integers(0, 256, (h, w), dtype=np.uint8), L.natural_like(w, h, seed + i),
-                    np.full((h, w), 255, np.uint8)][i % 3])
-    return np.stack(out)
-
-
 def _src(p, fr, seed=1):
     S = Region(fr.nbytes, p.get("src", 0), fr, seed)
     return S
@@ -383,47 +258,44 @@ def _ok(rc):
     _lib.check(rc, "dispatch row")
 
 
-def r_box(G, O, p, adaptive):
-    import test_gpu_parity as P
+def r_box(lib, O, p, adaptive):
     w, h, n, r = p["w"], p["h"], p["n"], p["r"]
     fr = frames(w, h, n, w + h + r)
     S, D = _src(p, fr), Region(fr.nbytes, p.get("dst", 0), seed=2)
     if adaptive:
-        rc, seen = traced(lambda: G.gs_b200_adaptive_threshold_batch(D.ptr, S.ptr, w, h, n, r, p["c"], _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_adaptive_threshold_batch(D.ptr, S.ptr, w, h, n, r, p["c"], stream()))
     else:
-        rc, seen = traced(lambda: G.gs_b200_blur_batch(D.ptr, S.ptr, w, h, n, r, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_blur_batch(D.ptr, S.ptr, w, h, n, r, stream()))
     _ok(rc)
     got = D.read("dst").reshape(n, h, w)
     _src_kept(S, fr)
     for i in range(n):
-        want = P.o_adaptive(O, fr[i], r, p["c"]) if adaptive else P.o_blur(O, fr[i], r)
+        want = L.o_adaptive(O, fr[i], r, p["c"]) if adaptive else L.o_blur(O, fr[i], r)
         assert np.array_equal(got[i], want), i
     return seen
 
 
-def r_blur_sobel(G, O, p):
-    import test_gpu_parity as P
+def r_blur_sobel(lib, O, p):
     w, h, n, r = p["w"], p["h"], p["n"], p["r"]
     fr = frames(w, h, n, w + h + r)
     S, D = _src(p, fr), Region(fr.nbytes, p.get("dst", 0), seed=2)
-    rc, seen = traced(lambda: G.gs_b200_blur_sobel_batch(D.ptr, S.ptr, w, h, n, r, _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_blur_sobel_batch(D.ptr, S.ptr, w, h, n, r, stream()))
     _ok(rc)
     got, fill = D.read("dst").reshape(n, h, w), D.before().reshape(n, h, w)
     _src_kept(S, fr)
     for i in range(n):
         want = fill[i].copy()                                   # the untouched 1-px frame keeps dst's bytes
-        O.gso_sobel(L.ptr(want), L.ptr(P.o_blur(O, fr[i], r)), w, h)
+        O.gso_sobel(L.ptr(want), L.ptr(L.o_blur(O, fr[i], r)), w, h)
         assert np.array_equal(got[i], want), i
     return seen
 
 
-def r_stencil(G, O, p, op):
-    import test_gpu_parity as P
+def r_stencil(lib, O, p, op):
     w, h, n = p["w"], p["h"], p["n"]
     fr = frames(w, h, n, w + h)
     S, D = _src(p, fr), Region(fr.nbytes, p.get("dst", 0), seed=2)
-    fn = {"sobel": G.gs_b200_sobel_batch, "erode": G.gs_b200_erode_batch, "dilate": G.gs_b200_dilate_batch}[op]
-    rc, seen = traced(lambda: fn(D.ptr, S.ptr, w, h, n, _stream()))
+    fn = {"sobel": lib.gs_b200_sobel_batch, "erode": lib.gs_b200_erode_batch, "dilate": lib.gs_b200_dilate_batch}[op]
+    rc, seen = traced(lambda: fn(D.ptr, S.ptr, w, h, n, stream()))
     _ok(rc)
     got, fill = D.read("dst").reshape(n, h, w), D.before().reshape(n, h, w)
     _src_kept(S, fr)
@@ -432,64 +304,62 @@ def r_stencil(G, O, p, op):
             want = fill[i].copy()
             O.gso_sobel(L.ptr(want), L.ptr(fr[i]), w, h)
         else:
-            want = P.o_morph(O, fr[i], op == "dilate")
+            want = L.o_morph(O, fr[i], op == "dilate")
         assert np.array_equal(got[i], want), i
     return seen
 
 
-def r_resample(G, O, p, op):
-    import test_gpu_parity as P
+def r_resample(lib, O, p, op):
     w, h, n = p["w"], p["h"], p["n"]
     dw, dh = (w // 2, h // 2) if op == "downsample" else (p["dw"], p["dh"])
     fr = frames(w, h, n, w + h + dw)
     S, D = _src(p, fr), Region(n * dw * dh, p.get("dst", 0), seed=2)
     if op == "downsample":
-        rc, seen = traced(lambda: G.gs_b200_downsample_batch(D.ptr, S.ptr, w, h, n, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_downsample_batch(D.ptr, S.ptr, w, h, n, stream()))
     else:
-        rc, seen = traced(lambda: G.gs_b200_resize_batch(D.ptr, dw, dh, S.ptr, w, h, n, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_resize_batch(D.ptr, dw, dh, S.ptr, w, h, n, stream()))
     _ok(rc)
     got = D.read("dst").reshape(n, dh, dw)
     _src_kept(S, fr)
     for i in range(n):
-        want = P.o_down(O, fr[i]) if op == "downsample" else P.o_resize(O, fr[i], dw, dh)
+        want = L.o_down(O, fr[i]) if op == "downsample" else L.o_resize(O, fr[i], dw, dh)
         assert np.array_equal(got[i], want), i
     return seen
 
 
-def r_integral(G, O, p):
-    import test_gpu_parity as P
+def r_integral(lib, O, p):
     w, h, n = p["w"], p["h"], p["n"]
     fr = frames(w, h, n, w + h + n)
     S, D = _src(p, fr), Region(4 * n * w * h, p.get("ii", 0), seed=2)
     if "env" in p:
         os.environ["GS_B200_INTEGRAL"] = p["env"]
     try:
-        rc, seen = traced(lambda: G.gs_b200_integral_batch(D.ptr, S.ptr, w, h, n, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_integral_batch(D.ptr, S.ptr, w, h, n, stream()))
     finally:
         os.environ.pop("GS_B200_INTEGRAL", None)
     _ok(rc)
     got = D.read("ii").view(np.uint32).reshape(n, h, w)
     _src_kept(S, fr)
     for i in range(n):
-        assert np.array_equal(got[i], P.o_integral(O, fr[i])), i
+        assert np.array_equal(got[i], L.o_integral(O, fr[i])), i
     return seen
 
 
-def r_histogram(G, O, p, op):
+def r_histogram(lib, O, p, op):
     w, h, n = p["w"], p["h"], p["n"]
     fr = frames(w, h, n, w + h)
     fr[n - 1] = np.random.default_rng(3).integers(0, 256, (h, w), dtype=np.uint8) // 64 * 64   # four bins only
     S = _src(p, fr)
     if op == "histogram":
         D = Region(4 * 256 * n, p.get("hist", 0), seed=2)
-        rc, seen = traced(lambda: G.gs_b200_histogram_batch(D.ptr, S.ptr, w, h, n, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_histogram_batch(D.ptr, S.ptr, w, h, n, stream()))
         _ok(rc)
         got = D.read("hist").view(np.uint32).reshape(n, 256)
         for i in range(n):
             assert np.array_equal(got[i], np.bincount(fr[i].ravel(), minlength=256)), i
     else:
         D = Region(n, 1, seed=2)
-        rc, seen = traced(lambda: G.gs_b200_otsu_threshold_batch(D.ptr, None, S.ptr, w, h, n, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_otsu_threshold_batch(D.ptr, None, S.ptr, w, h, n, stream()))
         _ok(rc)
         got = D.read("thresholds")
         for i in range(n):
@@ -498,18 +368,18 @@ def r_histogram(G, O, p, op):
     return seen
 
 
-def r_threshold(G, O, p, each):
+def r_threshold(lib, O, p, each):
     w, h, n = p["w"], p["h"], p["n"]
     fr = frames(w, h, n, w + h)
     S = _src(p, fr)                                            # in place
     if each:
         thr = np.array([100, 0, 250, 37, 255][:n], np.uint8)
         T = Region(n, 3, thr, seed=2)
-        rc, seen = traced(lambda: G.gs_b200_threshold_each_batch(S.ptr, w, h, n, T.ptr, p["offset"], _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_threshold_each_batch(S.ptr, w, h, n, T.ptr, p["offset"], stream()))
         T.read("thresholds")
         ts = [(int(t) + p["offset"]) & 255 for t in thr]
     else:
-        rc, seen = traced(lambda: G.gs_b200_threshold_batch(S.ptr, w, h, n, p["t"], _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_threshold_batch(S.ptr, w, h, n, p["t"], stream()))
         ts = [p["t"]] * n
     _ok(rc)
     got = S.read("img").reshape(n, h, w)
@@ -520,14 +390,14 @@ def r_threshold(G, O, p, each):
     return seen
 
 
-def r_filter(G, O, p):
+def r_filter(lib, O, p):
     w, h, n = p["w"], p["h"], p["n"]
     fr = frames(w, h, n, w + h)
     k, norm = L.filter_kernel(p["k"])
     S, D = _src(p, fr), Region(fr.nbytes, p.get("dst", 0), seed=2)
     ks = np.ascontiguousarray(k)
-    rc, seen = traced(lambda: G.gs_b200_filter_batch(D.ptr, S.ptr, w, h, n, ks.ctypes.data, ks.shape[1], ks.shape[0],
-                                                    norm, _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_filter_batch(D.ptr, S.ptr, w, h, n, ks.ctypes.data, ks.shape[1], ks.shape[0],
+                                                      norm, stream()))
     _ok(rc)
     got = D.read("dst").reshape(n, h, w)
     _src_kept(S, fr)
@@ -538,13 +408,13 @@ def r_filter(G, O, p):
     return seen
 
 
-def r_match_template(G, O, p):
+def r_match_template(lib, O, p):
     w, h, n, tw, th = p["w"], p["h"], p["n"], p["tw"], p["th"]
     fr = frames(w, h, n, w + h)
     tmpl = np.ascontiguousarray(fr[1, 10:10 + th, 20:20 + tw])
     rw, rh = w - tw + 1, h - th + 1
     S, T, D = _src(p, fr), Region(tmpl.nbytes, 0, tmpl, seed=3), Region(n * rw * rh, p.get("res", 0), seed=2)
-    rc, seen = traced(lambda: G.gs_b200_match_template_batch(D.ptr, S.ptr, w, h, n, T.ptr, tw, th, _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_match_template_batch(D.ptr, S.ptr, w, h, n, T.ptr, tw, th, stream()))
     _ok(rc)
     got = D.read("result").reshape(n, rh, rw)
     _src_kept(S, fr)
@@ -556,7 +426,7 @@ def r_match_template(G, O, p):
     return seen
 
 
-def r_find_best_match(G, O, p):
+def r_find_best_match(lib, O, p):
     rw, rh, n = p["w"], p["h"], p["n"]
     px = rw * rh
     assert px % 2 == 1
@@ -569,7 +439,7 @@ def r_find_best_match(G, O, p):
     maps[4, px // 2] = 254                               # interior
     maps[4, px // 2 + 1] = 254
     M, B = Region(maps.nbytes, p.get("res", 0), maps, seed=3), Region(8 * n, 0, seed=2)
-    rc, seen = traced(lambda: G.gs_b200_find_best_match_batch(B.ptr, M.ptr, rw, rh, n, _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_find_best_match_batch(B.ptr, M.ptr, rw, rh, n, stream()))
     _ok(rc)
     got = B.read("best").view(np.uint32).reshape(n, 2)
     M.read("result")
@@ -580,8 +450,7 @@ def r_find_best_match(G, O, p):
     return seen
 
 
-def r_fast(G, O, p, orb):
-    import test_gpu_parity as P
+def r_fast(lib, O, p, orb):
     w, h, n, t = p["w"], p["h"], p["n"], p["t"]
     nk = 400
     fr = frames(w, h, n, w + h)
@@ -590,8 +459,8 @@ def r_fast(G, O, p, orb):
     stale = np.zeros_like(fr) if orb else (rng.integers(0, 256, fr.shape) * (rng.random(fr.shape) < 0.02)).astype(np.uint8)
     S, SM = _src(p, fr), Region(fr.nbytes, p.get("score", 0), stale, seed=4)
     K, N = Region(48 * n * nk, 0, seed=5), Region(4 * n, 0, seed=6)
-    fn = G.gs_b200_orb_extract_batch if orb else G.gs_b200_fast_batch
-    rc, seen = traced(lambda: fn(S.ptr, w, h, n, SM.ptr, K.ptr, N.ptr, nk, t, _stream()))
+    fn = lib.gs_b200_orb_extract_batch if orb else lib.gs_b200_fast_batch
+    rc, seen = traced(lambda: fn(S.ptr, w, h, n, SM.ptr, K.ptr, N.ptr, nk, t, stream()))
     _ok(rc)
     counts = N.read("counts").view(np.uint32)
     kps = K.read("kps").view(np.uint32).reshape(n, nk, 12)
@@ -599,7 +468,7 @@ def r_fast(G, O, p, orb):
     _src_kept(S, fr)
     for i in range(n):
         so = stale[i].copy()
-        want = P.o_orb(O, fr[i], so, nk, t) if orb else P.o_fast(O, fr[i], so, nk, t)
+        want = L.o_orb(O, fr[i], so, nk, t) if orb else L.o_fast(O, fr[i], so, nk, t)
         got = np.ascontiguousarray(kps[i, :counts[i]]).view(L.KP_DTYPE).reshape(-1)
         assert got.tobytes() == want.tobytes(), (i, len(got), len(want))
         if not orb:
@@ -619,13 +488,12 @@ def _cascade(kind):
     return HostCascade(a)
 
 
-def r_lbp(G, O, p):
-    import test_gpu_parity as P
+def r_lbp(lib, O, p):
     w, h, n = p["w"], p["h"], p["n"]
     lena = np.load(os.path.join(L.ROOT, "tests", "golden", "lena_golden.npz"))["lena"]      # 128 x 128, faces found
     fr = np.stack([np.pad(np.roll(lena, 4 * i, axis=1), ((0, h - 128), (0, w - 128)), mode="edge") if i < 2 else
                    L.natural_like(w, h, 40 + i) for i in range(n)])
-    ii = np.stack([P.o_integral(O, f) for f in fr])
+    ii = np.stack([L.o_integral(O, f) for f in fr])
     cas = _cascade(p.get("cascade", "frontalface"))
     I = Region(ii.nbytes, p.get("ii", 0), ii, seed=3)
     mr = 1000
@@ -633,8 +501,8 @@ def r_lbp(G, O, p):
     if "big" in p:
         os.environ["GS_B200_LBP_BIG"] = p["big"]
     try:
-        rc, seen = traced(lambda: G.gs_b200_lbp_detect_batch(cas.ptr, I.ptr, w, h, n, RR.ptr, N.ptr, mr, 1.1, 1.0, 4.0,
-                                                            2, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_lbp_detect_batch(cas.ptr, I.ptr, w, h, n, RR.ptr, N.ptr, mr, 1.1, 1.0, 4.0,
+                                                              2, stream()))
     finally:
         os.environ.pop("GS_B200_LBP_BIG", None)
     _ok(rc)
@@ -642,7 +510,7 @@ def r_lbp(G, O, p):
     rects = RR.read("rects").view(np.uint32).reshape(n, mr, 4)
     I.read("ii")
     for i in range(n):
-        want = P.o_detect(O, cas, ii[i], mr, 1.1, 1.0, 4.0, 2)
+        want = L.o_detect(O, cas, ii[i], mr, 1.1, 1.0, 4.0, 2)
         assert np.ascontiguousarray(rects[i, :counts[i]]).tobytes() == want.tobytes(), (i, counts[i], len(want))
     assert counts.sum() > 0
     return seen
@@ -655,12 +523,12 @@ def _o_blobs(O, a, nb):
     return labels, blobs[:m]
 
 
-def r_blobs(G, O, p):
+def r_blobs(lib, O, p):
     w, h, n, nb = p["w"], p["h"], p["n"], 300
     fr = np.stack([L.binary_like(w, h, 50 + i) for i in range(n)])
     S, LB = _src(p, fr), Region(2 * n * w * h, 2, seed=2)
     B, N = Region(32 * n * nb, 0, seed=3), Region(4 * n, 0, seed=4)
-    rc, seen = traced(lambda: G.gs_b200_blobs_batch(S.ptr, w, h, n, LB.ptr, B.ptr, N.ptr, nb, _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_blobs_batch(S.ptr, w, h, n, LB.ptr, B.ptr, N.ptr, nb, stream()))
     _ok(rc)
     labels = LB.read("labels").view(np.uint16).reshape(n, h, w)
     blobs, counts = B.read("blobs").view(L.BLOB_DTYPE).reshape(n, nb), N.read("counts").view(np.uint32)
@@ -672,14 +540,14 @@ def r_blobs(G, O, p):
     return seen
 
 
-def r_blob_corners(G, O, p):
+def r_blob_corners(lib, O, p):
     w, h = p["w"], p["h"]
     a = L.binary_like(w, h, 7)
     labels, blobs = _o_blobs(O, a, 300)
     j = int(np.argmax(blobs["area"]))
     S, LB = _src(p, a), Region(labels.nbytes, 2, labels, seed=2)
     B, CO = Region(32, 0, blobs[j:j + 1], seed=3), Region(32, 0, seed=4)
-    rc, seen = traced(lambda: G.gs_b200_blob_corners(S.ptr, w, h, LB.ptr, B.ptr, CO.ptr, _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_blob_corners(S.ptr, w, h, LB.ptr, B.ptr, CO.ptr, stream()))
     _ok(rc)
     got = CO.read("corners").view(np.uint32).reshape(4, 2)
     want = np.zeros((4, 2), np.uint32)
@@ -688,19 +556,19 @@ def r_blob_corners(G, O, p):
     return seen
 
 
-def r_perspective(G, O, p):
+def r_perspective(lib, O, p):
     w, h, n, dw, dh = p["w"], p["h"], p["n"], p["dw"], p["dh"]
     fr = frames(w, h, n, w + h)
     quads = np.random.default_rng(5).integers(0, 140, (n, 4, 2)).astype(np.uint32)
     S, D = _src(p, fr), Region(n * dw * dh, p.get("dst", 0), seed=2)
     if p.get("per_frame"):
         Q = Region(quads.nbytes, 0, quads, seed=3)
-        rc, seen = traced(lambda: G.gs_b200_perspective_correct_batch(D.ptr, dw, dh, S.ptr, w, h, n, Q.ptr, 1, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_perspective_correct_batch(D.ptr, dw, dh, S.ptr, w, h, n, Q.ptr, 1, stream()))
     else:
         quads[:] = quads[0]
         q0 = np.ascontiguousarray(quads[0])
-        rc, seen = traced(lambda: G.gs_b200_perspective_correct_batch(D.ptr, dw, dh, S.ptr, w, h, n, q0.ctypes.data, 0,
-                                                                     _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_perspective_correct_batch(D.ptr, dw, dh, S.ptr, w, h, n, q0.ctypes.data, 0,
+                                                                       stream()))
     _ok(rc)
     got = D.read("dst").reshape(n, dh, dw)
     _src_kept(S, fr)
@@ -711,8 +579,7 @@ def r_perspective(G, O, p):
     return seen
 
 
-def r_match_orb(G, O, p):
-    import test_gpu_parity as P
+def r_match_orb(lib, O, p):
     n, s1, s2, mm = p["n"], 130, 90, 150
     rng = np.random.default_rng(16)
     sets = [L.desc_sets(rng, n1, n2) for n1, n2 in ((120, 90), (7, 0), (130, 61))][:n]
@@ -723,35 +590,35 @@ def r_match_orb(G, O, p):
         k1[i, :len(a)], k2[i, :len(b)] = a, b
     K1, K2, C1, C2 = Region(k1.nbytes, 0, k1, 1), Region(k2.nbytes, 0, k2, 2), Region(4 * n, 0, c1, 3), Region(4 * n, 0, c2, 4)
     M, MC = Region(12 * n * mm, 0, seed=5), Region(4 * n, 0, seed=6)
-    rc, seen = traced(lambda: G.gs_b200_match_orb_batch(K1.ptr, C1.ptr, s1, K2.ptr, C2.ptr, s2, n, M.ptr, MC.ptr, mm, 60.0,
-                                                       _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_match_orb_batch(K1.ptr, C1.ptr, s1, K2.ptr, C2.ptr, s2, n, M.ptr, MC.ptr, mm, 60.0,
+                                                         stream()))
     _ok(rc)
     counts, m = MC.read("counts").view(np.uint32), M.read("matches").view(np.uint32).reshape(n, mm, 3)
     for i, (a, b) in enumerate(sets):
-        want = P._o_match(O, a, b, mm, 60.0)
+        want = L.o_match(O, a, b, mm, 60.0)
         assert counts[i] == len(want) and np.ascontiguousarray(m[i, :counts[i]]).tobytes() == want.tobytes(), i
     return seen
 
 
 RUN = {
-    "blur": lambda G, O, p: r_box(G, O, p, False),
-    "adaptive": lambda G, O, p: r_box(G, O, p, True),
+    "blur": lambda lib, O, p: r_box(lib, O, p, False),
+    "adaptive": lambda lib, O, p: r_box(lib, O, p, True),
     "blur_sobel": r_blur_sobel,
-    "sobel": lambda G, O, p: r_stencil(G, O, p, "sobel"),
-    "erode": lambda G, O, p: r_stencil(G, O, p, "erode"),
-    "dilate": lambda G, O, p: r_stencil(G, O, p, "dilate"),
-    "downsample": lambda G, O, p: r_resample(G, O, p, "downsample"),
-    "resize": lambda G, O, p: r_resample(G, O, p, "resize"),
+    "sobel": lambda lib, O, p: r_stencil(lib, O, p, "sobel"),
+    "erode": lambda lib, O, p: r_stencil(lib, O, p, "erode"),
+    "dilate": lambda lib, O, p: r_stencil(lib, O, p, "dilate"),
+    "downsample": lambda lib, O, p: r_resample(lib, O, p, "downsample"),
+    "resize": lambda lib, O, p: r_resample(lib, O, p, "resize"),
     "integral": r_integral,
-    "histogram": lambda G, O, p: r_histogram(G, O, p, "histogram"),
-    "otsu": lambda G, O, p: r_histogram(G, O, p, "otsu"),
-    "threshold": lambda G, O, p: r_threshold(G, O, p, False),
-    "threshold_each": lambda G, O, p: r_threshold(G, O, p, True),
+    "histogram": lambda lib, O, p: r_histogram(lib, O, p, "histogram"),
+    "otsu": lambda lib, O, p: r_histogram(lib, O, p, "otsu"),
+    "threshold": lambda lib, O, p: r_threshold(lib, O, p, False),
+    "threshold_each": lambda lib, O, p: r_threshold(lib, O, p, True),
     "filter": r_filter,
     "match_template": r_match_template,
     "find_best_match": r_find_best_match,
-    "fast": lambda G, O, p: r_fast(G, O, p, False),
-    "orb": lambda G, O, p: r_fast(G, O, p, True),
+    "fast": lambda lib, O, p: r_fast(lib, O, p, False),
+    "orb": lambda lib, O, p: r_fast(lib, O, p, True),
     "lbp": r_lbp,
     "blobs": r_blobs,
     "blob_corners": r_blob_corners,
@@ -766,14 +633,5 @@ def test_every_row_has_a_runner():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("op,kernels,p", [pytest.param(op, k, p, id=row_id(op, p)) for op, k, p in ROWS])
-def test_dispatch_row(G, witness, op, kernels, p):
-    seen = RUN[op](G, L.oracle(), p)
-    if witness and not seen:
-        # every row launches at least one kernel, so an empty list is a profiler session that delivered no device
-        # records (2 of 162 sessions in one run on the H100, their neighbours witnessed): the row runs once more
-        seen = RUN[op](G, L.oracle(), p)
-    print("\n%s: launched %s" % (row_id(op, p), " ".join(sorted(seen))))
-    if not witness:
-        pytest.skip("parity holds; kineto recorded no kernel events for the probe launch, so the path is not witnessed")
-    missing = [k for k in kernels if kernel_id(k) not in seen]
-    assert not missing, "expected %s, launched %s" % (missing, sorted(seen))
+def test_dispatch_row(lib, O, witness, op, kernels, p):
+    witnessed(witness, lambda: RUN[op](lib, O, p), kernels, row_id(op, p))

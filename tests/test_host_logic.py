@@ -41,10 +41,10 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_sass_is_sm90a_with_tma():
-    """the shipped cubin targets sm_90a and the tiled kernels really use TMA (UTMALDG)"""
-    from grayskull_b200 import _lib
-    out = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_90a" in out
+    """every kernel of the shipped library is sm_90a code and the tiled kernels really use TMA (UTMALDG)"""
+    sass = L.sass_functions()
+    assert sass and all(body.startswith("code for sm_90a\n") for body in sass.values())
+    out = "".join(sass.values())
     assert "UTMALDG" in out and "SYNCS" in out
     assert "VIMNMX3.U16x2" in out and "HMNMX2" in out      # packed-lane arithmetic, not scalar bytes
 
@@ -279,6 +279,47 @@ def test_box_mid_row_walk_matches_direct_window_sums():
                 want = np.array([Cp[c + 1: c + 2 * r + 2].sum() for c in range(R8, R8 + len(got))])
                 assert np.array_equal(got, want), (r, w_img, strip)
                 assert len(got) >= min(outw, w_img - (xs + R8)), (r, w_img, strip)   # every in-image output is produced
+
+
+def _window_sums(V, R):
+    """box.cu window_sums<R> (k_box_tma) on Python ints, mod 2^32: V = 12 pair words (lo column 2m, hi 2m+1)"""
+    M = 0xFFFFFFFF
+    odd = R & 1
+    NP = R if odd else R + 1
+    M0 = (8 - R + 1) // 2 if odd else (8 - R) // 2
+    ps = sum(V[M0:M0 + NP]) & M
+    T = []
+    for p in range(4):
+        m = M0 + p
+        x16 = ((ps * 0x10001) & M) >> 16
+        if odd:
+            edge = (V[m - 1] >> 16) | ((V[m + NP] & 0xFFFF) << 16)      # prmt(V[m-1], V[m+NP], 0x5432)
+            T.append((x16 * 0x10001 + edge) & M)
+        else:
+            sub = (V[m + R] >> 16) | ((V[m] & 0xFFFF) << 16)           # prmt(V[m+R], V[m], 0x5432)
+            T.append((x16 * 0x10001 - sub) & M)
+        if p < 3:
+            ps = (ps + V[m + NP] - V[m]) & M
+    return T
+
+
+@pytest.mark.parametrize("R", range(1, 8))
+def test_halo_lane_pixels_ignore_missing_words(R):
+    """box.cu window_sums<R>, k_box_tma's horizontal step: a lane's 12 pair words V are the column sums of columns
+    x-8 .. x+15, the outer four on each side shuffled from its neighbour lanes.  The words of a missing neighbour (the
+    shuffles of lanes 0 and 31 wrap to their own words: V[0..3] in lane 0, V[8..11] in lane 31) reach only the pixels on
+    their side: lane 0's pixel 7 and lane 31's pixel 0 are still the window sums of the true columns.  (k_box_tma
+    stores lanes 1..30 only; the test pins window_sums' data flow.)"""
+    rng = np.random.default_rng(R)
+    top = (2 * R + 1) * 255
+    for _ in range(2000):
+        s = rng.integers(0, top + 1, 24)                            # true column sums of columns x-8 .. x+15
+        true = [int(s[2 * m]) | int(s[2 * m + 1]) << 16 for m in range(12)]
+        junk = [int(a) | int(b) << 16 for a, b in rng.integers(0, top + 1, (4, 2))]
+        lane0 = _window_sums(junk + true[4:], R)
+        assert lane0[3] >> 16 == int(s[15 - R:16 + R].sum()), R    # pixel 7 = column x+7 = index 15
+        lane31 = _window_sums(true[:8] + junk, R)
+        assert lane31[0] & 0xFFFF == int(s[8 - R:9 + R].sum()), R   # pixel 0 = column x = index 8
 
 
 def test_filter_magic_division_is_exact():

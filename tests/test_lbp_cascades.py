@@ -24,11 +24,10 @@ kills windows, some windows pass with sum == threshold exactly, and every frame 
     model's mutants (reversed or pairwise stage sums, nsub ignored, window transposed, `<=` for `<`, corners beyond
     the window read as 0), each of which must change the hits of the cascade built to catch it.
   * GPU: every cascade through every scan kernel that can take it, bit-exact against the oracle, each path witnessed
-    under torch.profiler as in test_dispatch_paths.py; k_lbp_window_one at ~500 positions per cascade; and the plan
+    under torch.profiler (tests/_gpu.py); k_lbp_window_one at ~500 positions per cascade; and the plan
     cache (keyed by the cascade's contents) across cascades that differ in one threshold or one subset bit, and across
     in-place edits of one cascade.
 """
-import ctypes as C
 import functools
 import os
 
@@ -36,8 +35,7 @@ import numpy as np
 import pytest
 
 import _libs as L
-from test_dispatch_paths import Region, kernel_id, traced, witness  # noqa: F401  (witness is a fixture)
-from test_gpu_parity import o_detect, o_integral
+from _gpu import O, Region, lib, stream, traced, witness, witnessed  # noqa: F401
 
 F32 = np.float32
 CAL = dict(sf=1.25, mn=1.0, step=2)        # the ladder the thresholds are calibrated on (max_scale per case)
@@ -345,7 +343,7 @@ class Case:
 
 
 def integrals(O, imgs):
-    return np.stack([o_integral(O, f) for f in imgs])
+    return np.stack([L.o_integral(O, f) for f in imgs])
 
 
 @functools.lru_cache(maxsize=None)
@@ -354,11 +352,6 @@ def case(name):
 
 
 NAMES = list(SPECS)
-
-
-@pytest.fixture(scope="module")
-def O():
-    return L.oracle()
 
 
 # ---- CPU: calibration, definedness, model == oracle == reference, mutants ----------------------------------------
@@ -556,21 +549,7 @@ def test_mutant_changes_hits(name, mutant):
 
 
 # ---- GPU ---------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def G():
-    import torch
-    import grayskull_b200 as g
-    assert torch.cuda.is_available()
-    g.lib().gs_b200_set_device(0)
-    return g.lib()
-
-
-def _stream():
-    import torch
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def gpu_detect(G, cas, ii, mr, sf, mn, mx, step, off=0, env=None, generic=False):
+def gpu_detect(lib, cas, ii, mr, sf, mn, mx, step, off=0, env=None, generic=False):
     """gs_b200_lbp_detect_batch on the (n, h, w) tables at byte offset `off`, under torch.profiler -> (rects per
     frame, launched kernels)"""
     from grayskull_b200 import _lib
@@ -580,15 +559,15 @@ def gpu_detect(G, cas, ii, mr, sf, mn, mx, step, off=0, env=None, generic=False)
     env = env or {}
     os.environ.update(env)
     if generic:
-        G.gs_b200_force_generic(1)
+        lib.gs_b200_force_generic(1)
     try:
-        rc, seen = traced(lambda: G.gs_b200_lbp_detect_batch(cas.ptr, I.ptr, w, h, n, RR.ptr, N.ptr, mr, sf, mn, mx,
-                                                            step, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_lbp_detect_batch(cas.ptr, I.ptr, w, h, n, RR.ptr, N.ptr, mr, sf, mn, mx,
+                                                              step, stream()))
     finally:
         for k in env:
             os.environ.pop(k, None)
         if generic:
-            G.gs_b200_force_generic(0)
+            lib.gs_b200_force_generic(0)
     _lib.check(rc, "lbp_detect_batch")
     counts = N.read("counts").view(np.uint32)
     rects = RR.read("rects").view(np.uint32).reshape(n, mr, 4)
@@ -636,55 +615,35 @@ def padded(a, nfeatures=5200):
     return p
 
 
-def _run_witnessed(witness, run, check, kernel, tries=3):
-    """run() -> (result, launched kernels); check(result) asserts parity.  The profiler sometimes loses device records:
-    a whole session (about 1 in 100 on the H100, sometimes two in a row) or a single kernel of a session whose other
-    launches it records.  So a run whose list misses `kernel` runs again, checked again, up to `tries` times; a path
-    that really launches another kernel misses it every time and fails in _witnessed."""
-    seen = set()
-    for _ in range(tries):
-        out, got = run()
-        check(out)
-        seen = got
-        if not witness or kernel_id(kernel) in seen:
-            break
-    return seen
-
-
-def _witnessed(witness, seen, kernel):
-    if not witness:
-        pytest.skip("parity holds; kineto recorded no kernel events for the probe launch, so the path is not witnessed")
-    assert kernel_id(kernel) in seen, "expected %s, launched %s" % (kernel, sorted(seen))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,path", GPU_CASES, ids=["%s-%s" % c for c in GPU_CASES])
-def test_detect_path(G, O, witness, name, path):
+def test_detect_path(lib, O, witness, name, path):
     """3 frames per batch through the path's kernel, counts and rects bit-exact against the oracle"""
     cs = case(name)
     _, off, _, env, generic, kernel = PATHS[path]
     a = padded(cs.arrays) if path == "big_tables" else cs.arrays
     cas = cs.cascade(a)
-    total, seen_all = 0, set()
+    scans = []
     for sf, mn, mx, step, w, h in gpu_scans(cs, path):
         assert PATHS[path][2] == 0 or w % 8
         ii = integrals(O, frames_at(w, h)[0])
-        want = [o_detect(O, cas, ii[i], BIG_MR, sf, mn, mx, step) for i in range(len(ii))]
-        total += sum(len(r) for r in want)
+        scans.append((sf, mn, mx, step, ii, [L.o_detect(O, cas, t, BIG_MR, sf, mn, mx, step) for t in ii]))
+    assert sum(len(r) for *_, want in scans for r in want) > 0
 
-        def check(got):
+    def run():
+        seen = set()
+        for sf, mn, mx, step, ii, want in scans:
+            got, s = gpu_detect(lib, cas, ii, BIG_MR, sf, mn, mx, step, off, env, generic)
             for i in range(len(ii)):
                 assert got[i].tobytes() == want[i].tobytes(), (sf, mn, step, i, len(got[i]), len(want[i]))
-        seen_all |= _run_witnessed(witness, lambda: gpu_detect(G, cas, ii, BIG_MR, sf, mn, mx, step, off, env, generic),
-                                   check, kernel)
-    print("\n%s-%s: launched %s" % (name, path, " ".join(sorted(seen_all))))
-    assert total > 0
-    _witnessed(witness, seen_all, kernel)
+            seen |= s
+        return seen
+    witnessed(witness, run, [kernel], "%s-%s" % (name, path))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", NAMES)
-def test_window_one(G, O, witness, name):
+def test_window_one(lib, O, witness, name):
     """single-window gs_lbp_window (k_lbp_window_one) against gso_lbp_window, 500 positions per cascade and frame"""
     cs = case(name)
     cas = cs.cascade()
@@ -695,7 +654,7 @@ def test_window_one(G, O, witness, name):
         t = np.ascontiguousarray(ii[i])
         for x, y, s in pos:
             want = O.gso_lbp_window(cas.ptr, L.ptr(t), cs.w, cs.h, x, y, s)
-            assert G.gs_lbp_window(cas.ptr, L.ptr(t), cs.w, cs.h, x, y, s) == want, (i, x, y, s)
+            assert lib.gs_lbp_window(cas.ptr, L.ptr(t), cs.w, cs.h, x, y, s) == want, (i, x, y, s)
             hits += want
     assert 0 < hits < len(ii) * len(pos)
     x, y, s = pos[0]                                   # a hit of the calibration scan
@@ -703,19 +662,18 @@ def test_window_one(G, O, witness, name):
     want = O.gso_lbp_window(cas.ptr, L.ptr(t), cs.w, cs.h, x, y, s)
     assert want == 1
 
-    def check(got):
+    def run():
+        got, seen = traced(lambda: lib.gs_lbp_window(cas.ptr, L.ptr(t), cs.w, cs.h, x, y, s))
         assert got == want
-    seen = _run_witnessed(witness, lambda: traced(lambda: G.gs_lbp_window(cas.ptr, L.ptr(t), cs.w, cs.h, x, y, s)),
-                          check, "gsb::k_lbp_window_one")
-    print("\n%s window: launched %s" % (name, " ".join(sorted(seen))))
-    _witnessed(witness, seen, "gsb::k_lbp_window_one")
+        return seen
+    witnessed(witness, run, ["gsb::k_lbp_window_one"], "%s window" % name)
 
 
 def _flip_that_matters(O, cs, ii):
     """(word, bit): one subset bit of a stage-0 weak whose flip changes the hits of frame 0"""
     a = cs.arrays
     sf, mn, mx, step, _, _ = cs.cal_scans[0]
-    base = o_detect(O, cs.cascade(), ii[0], BIG_MR, sf, mn, mx, step)
+    base = L.o_detect(O, cs.cascade(), ii[0], BIG_MR, sf, mn, mx, step)
     for r in base[:20]:
         f = scaled_features(a, next(s for s, ww, wh in ladder(*a["window"], *ii.shape[1:][::-1], sf, mn, mx)
                                     if (ww, wh) == (r["w"], r["h"])))
@@ -727,14 +685,14 @@ def _flip_that_matters(O, cs, ii):
             word, bit = int(a["weak_subset_offset"][wi]) + (code >> 5), code & 31
             b = {k: v.copy() for k, v in a.items()}
             b["subsets"][word] ^= np.uint32(1 << bit).view(np.int32)
-            if o_detect(O, cs.cascade(b), ii[0], BIG_MR, sf, mn, mx, step).tobytes() != base.tobytes():
+            if L.o_detect(O, cs.cascade(b), ii[0], BIG_MR, sf, mn, mx, step).tobytes() != base.tobytes():
                 return word, bit
     raise AssertionError("no subset bit of stage 0 changes the hits")
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("step", [2, 3])
-def test_plan_cache_follows_the_cascade(G, O, step):
+def test_plan_cache_follows_the_cascade(lib, O, step):
     """cascades that differ in one threshold, then in one subset bit, alternate; then one cascade is edited in place
     (same struct, same pointer) between calls.  Every call's hits are those of the cascade as it is at that call."""
     cs = case("short2")
@@ -749,8 +707,8 @@ def test_plan_cache_follows_the_cascade(G, O, step):
     args = (BIG_MR, CAL["sf"], CAL["mn"], cs.mx, step)
 
     def check(cas):
-        got, _ = gpu_detect(G, cas, ii, *args)
-        want = [o_detect(O, cas, ii[i], *args) for i in range(len(ii))]
+        got, _ = gpu_detect(lib, cas, ii, *args)
+        want = [L.o_detect(O, cas, ii[i], *args) for i in range(len(ii))]
         for i in range(len(ii)):
             assert got[i].tobytes() == want[i].tobytes(), (i, len(got[i]), len(want[i]))
         return b"".join(w.tobytes() for w in want)

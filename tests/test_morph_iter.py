@@ -4,16 +4,15 @@ The kernels rest on one identity: N passes of the reference's 3x3 op (min / max 
 neighbourhood) give the min / max over the in-image pixels of the (2N+1)^2 square, i.e. a clipped row window followed
 by a clipped column window.  The CPU tests pin that identity on the oracle (and on the reference build when present)
 and check the TMA kernels' SASS; the GPU tests check both dispatch paths bit for bit against iterated gso_morph."""
-import ctypes as C
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
 import _libs as L
+from _gpu import G, dev  # noqa: F401
 
 SHAPES = [(1, 1), (7, 1), (1, 7), (2, 2), (5, 3), (17, 9), (33, 40)]   # (w, h)
 
@@ -69,18 +68,8 @@ def test_iterated_reference_is_the_clipped_square(w, h):
                 assert np.array_equal(x, separable(a, dil, n)), (w, h, dil, n)
 
 
-def _functions(sass):
-    parts = re.split(r"^\s*Function : (\S+)\s*$", sass, flags=re.M)
-    return dict(zip(parts[1::2], parts[2::2]))
-
-
 def test_morph_tma_sass():
-    from grayskull_b200 import _lib
-    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(tool):
-        pytest.skip("cuobjdump not found")
-    out = subprocess.run([tool, "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    k = {name: body for name, body in _functions(out).items() if "k_morph_tma" in name}
+    k = {name: body for name, body in L.sass_functions().items() if "k_morph_tma" in name}
     assert len(k) == 30, sorted(k)                            # N = 2..16, erode and dilate
     for name, body in k.items():
         assert "UTMALDG" in body and "VIMNMX3.U16x2" in body, name
@@ -88,21 +77,6 @@ def test_morph_tma_sass():
 
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def G():
-    import torch
-    import grayskull_b200 as g
-    from grayskull_b200 import api
-    assert torch.cuda.is_available()
-    g.lib().gs_b200_set_device(0)
-    return api
-
-
-def dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
 def run(G, frames, dil, iters, offset=0):
     """frames (n, h, w) through the new entry, dst pre-filled with random bytes; `offset` shifts both bases"""
     import torch

@@ -257,23 +257,6 @@ def test_diff_match_orb():
         assert a == b and mr[:a].tobytes() == mo[:b].tobytes(), (n1, n2, mm, md, a, b)
 
 
-def otsu_images(rng):
-    """bimodal, flat, two-level, dark-heavy, noise and near-tie images: exercises wb == 0 skips, the wf == 0
-    break and fp32 ties in varBetween"""
-    out = []
-    for (w, h) in ((3, 3), (64, 48), (257, 31), (640, 480), (1, 1), (5, 1)):
-        out.append(rng.integers(0, 256, (h, w), dtype=np.uint8))
-        a = np.where(rng.random((h, w)) < 0.3, rng.normal(60, 12, (h, w)), rng.normal(190, 20, (h, w)))
-        out.append(np.clip(a, 0, 255).astype(np.uint8))
-        out.append(np.full((h, w), int(rng.integers(0, 256)), np.uint8))
-        b = np.full((h, w), 10, np.uint8); b.flat[:: max(1, (w * h) // 7)] = 250
-        out.append(b)
-        out.append((rng.integers(0, 2, (h, w)) * 255).astype(np.uint8))
-        out.append(rng.integers(100, 104, (h, w), dtype=np.uint8))
-    out.append(L.natural_like(1920, 1080, 3))
-    return out
-
-
 def test_testc_histogram_threshold_otsu():
     """the literal vectors of the reference's test.c:150-196"""
     a = np.array([[0, 50, 100], [50, 100, 150], [100, 150, 200]], np.uint8)
@@ -289,7 +272,7 @@ def test_testc_histogram_threshold_otsu():
 @needs_ref
 def test_diff_histogram_otsu_threshold():
     R = L.ref(); rng = np.random.default_rng(8)
-    for a in otsu_images(rng):
+    for a in L.otsu_images(rng):
         h, w = a.shape
         hr = np.zeros(256, np.uint32); ho = np.zeros(256, np.uint32)
         R.gs_histogram(L.img(a), L.ptr(hr)); O.gso_histogram(L.ptr(a), w, h, L.ptr(ho))

@@ -25,8 +25,7 @@ import numpy as np
 import pytest
 
 import _libs as L
-import test_gpu_parity as P
-from test_dispatch_paths import G, Region, _stream, frames, kernel_id, traced, witness  # noqa: F401
+from _gpu import Region, frames, lib, stream, traced, witness, witnessed  # noqa: F401
 
 INT_MIN, INT_MAX, UINT_MAX = -2 ** 31, 2 ** 31 - 1, 2 ** 32 - 1
 O = L.oracle()
@@ -36,18 +35,6 @@ needs_ref = pytest.mark.skipif(not L.have_ref(), reason="oracle/_ref not built")
 def _ok(rc):
     from grayskull_b200 import _lib
     _lib.check(rc, "extreme-parameter case")
-
-
-def _witnessed(witness, what, run, kernels):
-    """run() makes the calls, checks parity and returns the launched kernels; the case's kernels must be among them"""
-    seen = run()
-    if witness and not seen:    # a profiler session that delivered no device records: once more (test_dispatch_paths)
-        seen = run()
-    print("\n%s: launched %s" % (what, " ".join(sorted(seen))))
-    if not witness:
-        pytest.skip("parity holds; kineto recorded no kernel events for the probe launch, so the path is not witnessed")
-    missing = [k for k in kernels if kernel_id(k) not in seen]
-    assert not missing, "expected %s, launched %s" % (missing, sorted(seen))
 
 
 def _cid(v):
@@ -116,7 +103,7 @@ def test_ref_adaptive_c_extremes():
         for r in (0, 1, 2, 5, 9):
             for c in C_VALUES:
                 d = np.empty_like(a); R.gs_adaptive_threshold(L.img(d), L.img(a), r, c)
-                assert np.array_equal(d, P.o_adaptive(O, a, r, c)), (w, h, r, c)
+                assert np.array_equal(d, L.o_adaptive(O, a, r, c)), (w, h, r, c)
 
 
 def _adaptive_geoms():
@@ -131,7 +118,7 @@ def _adaptive_geoms():
 @pytest.mark.gpu
 @pytest.mark.parametrize("c", C_VALUES, ids=_cid)
 @pytest.mark.parametrize("name,w,h,r,kernel", [pytest.param(*g, id=g[0]) for g in _adaptive_geoms()])
-def test_adaptive_c(G, witness, name, w, h, r, kernel, c):
+def test_adaptive_c(lib, witness, name, w, h, r, kernel, c):
     if not lane_c_ok(c) and r <= 120:
         kernel = "gsb::k_box_wide<true>"
     fr = _c_frames(w, h, w + r)
@@ -148,14 +135,14 @@ def test_adaptive_c(G, witness, name, w, h, r, kernel, c):
                 got[i], seen = d, seen | s
         else:
             S, D = Region(fr.nbytes, 0, fr, 1), Region(fr.nbytes, 0, seed=2)
-            rc, seen = traced(lambda: G.gs_b200_adaptive_threshold_batch(D.ptr, S.ptr, w, h, n, r, c, _stream()))
+            rc, seen = traced(lambda: lib.gs_b200_adaptive_threshold_batch(D.ptr, S.ptr, w, h, n, r, c, stream()))
             _ok(rc)
             got = D.read("dst").reshape(n, h, w)
             assert np.array_equal(S.read("src"), fr.reshape(-1))
-        bad = [i for i in range(n) if not np.array_equal(got[i], P.o_adaptive(O, fr[i], r, c))]
+        bad = [i for i in range(n) if not np.array_equal(got[i], L.o_adaptive(O, fr[i], r, c))]
         assert not bad, "frames %s (random, natural, zeros, 255) differ from the oracle at c = %d" % (bad, c)
         return seen
-    _witnessed(witness, "adaptive-%s-c%s" % (name, _cid(c)), run, [kernel])
+    witnessed(witness, run, [kernel], "adaptive-%s-c%s" % (name, _cid(c)))
 
 
 # ---- b. thresholds ---------------------------------------------------------------------------------------------------
@@ -183,31 +170,31 @@ def _thr_geoms():
 @pytest.mark.gpu
 @pytest.mark.parametrize("t", THRESH, ids=_cid)
 @pytest.mark.parametrize("name,w,h,kernel", [pytest.param(*g, id=g[0]) for g in _thr_geoms()])
-def test_threshold_extremes(G, witness, name, w, h, kernel, t):
+def test_threshold_extremes(lib, witness, name, w, h, kernel, t):
     fr = frames(w, h, 3, w + h)
 
     def run():
         S = Region(fr.nbytes, 0, fr, 1)
-        rc, seen = traced(lambda: G.gs_b200_threshold_batch(S.ptr, w, h, 3, t, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_threshold_batch(S.ptr, w, h, 3, t, stream()))
         _ok(rc)
         got = S.read("img").reshape(3, h, w)
         for i in range(3):
             want = fr[i].copy(); O.gso_threshold(L.ptr(want), w, h, t & 0xFF)
             assert np.array_equal(got[i], want), i
         return seen
-    _witnessed(witness, "threshold-%s-t%s" % (name, _cid(t)), run, [kernel])
+    witnessed(witness, run, [kernel], "threshold-%s-t%s" % (name, _cid(t)))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("offset", OFFSETS, ids=_cid)
 @pytest.mark.parametrize("name,w,h,kernel", [pytest.param(*g, id=g[0]) for g in _thr_geoms()])
-def test_threshold_each_extremes(G, witness, name, w, h, kernel, offset):
+def test_threshold_each_extremes(lib, witness, name, w, h, kernel, offset):
     n = len(EACH)
     fr = frames(w, h, n, w + h + 1)
 
     def run():
         S, T = Region(fr.nbytes, 0, fr, 1), Region(n, 3, EACH, seed=2)
-        rc, seen = traced(lambda: G.gs_b200_threshold_each_batch(S.ptr, w, h, n, T.ptr, offset, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_threshold_each_batch(S.ptr, w, h, n, T.ptr, offset, stream()))
         _ok(rc)
         T.read("thresholds")
         got = S.read("img").reshape(n, h, w)
@@ -215,7 +202,7 @@ def test_threshold_each_extremes(G, witness, name, w, h, kernel, offset):
             want = fr[i].copy(); O.gso_threshold(L.ptr(want), w, h, (int(EACH[i]) + offset) % 256)  # (uint8_t)(t + off)
             assert np.array_equal(got[i], want), (i, int(EACH[i]))
         return seen
-    _witnessed(witness, "threshold_each-%s-off%s" % (name, _cid(offset)), run, [kernel])
+    witnessed(witness, run, [kernel], "threshold_each-%s-off%s" % (name, _cid(offset)))
 
 
 # ---- c. filter -------------------------------------------------------------------------------------------------------
@@ -296,10 +283,10 @@ def test_ref_filter_extremes():
             assert np.array_equal(d, want), (w, h, kw, kh, norm)
 
 
-def _run_filter(G, fr, k, kw, kh, norm):
+def _run_filter(lib, fr, k, kw, kh, norm):
     n, h, w = fr.shape
     S, D = Region(fr.nbytes, 0, fr, 1), Region(fr.nbytes, 0, seed=2)
-    rc, seen = traced(lambda: G.gs_b200_filter_batch(D.ptr, S.ptr, w, h, n, _kptr(k), kw, kh, norm, _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_filter_batch(D.ptr, S.ptr, w, h, n, _kptr(k), kw, kh, norm, stream()))
     _ok(rc)
     got = D.read("dst").reshape(n, h, w)
     assert np.array_equal(S.read("src"), fr.reshape(-1))
@@ -312,25 +299,25 @@ def _run_filter(G, fr, k, kw, kh, norm):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid,kname,norm", [pytest.param(*c, id=c[0]) for c in _filter3_cases()])
-def test_filter3_norm_extremes(G, witness, cid, kname, norm):
+def test_filter3_norm_extremes(lib, witness, cid, kname, norm):
     k = KERNELS3[kname]
     route = filter3_route(k, norm)
     kernel = "gsb::k_filter3<%s>" % route if route else "gsb::k_filter_generic"
     fr = frames(272, 41, 3, 7)
-    _witnessed(witness, "filter-" + cid, lambda: _run_filter(G, fr, k, 3, 3, norm), [kernel])
+    witnessed(witness, lambda: _run_filter(lib, fr, k, 3, 3, norm), [kernel], "filter-" + cid)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,w,h,k,kw,kh", [pytest.param(*c, id=c[0]) for c in _shape_kernels()])
-def test_filter_shapes(G, witness, name, w, h, k, kw, kh):
+def test_filter_shapes(lib, witness, name, w, h, k, kw, kh):
     fr = frames(w, h, 3, w + kw + kh)
 
     def run():
         seen = set()
         for norm in (1, 7, UINT_MAX):
-            seen |= _run_filter(G, fr, k, kw, kh, norm)
+            seen |= _run_filter(lib, fr, k, kw, kh, norm)
         return seen
-    _witnessed(witness, "filter-" + name, run, ["gsb::k_filter_generic"])
+    witnessed(witness, run, ["gsb::k_filter_generic"], "filter-" + name)
 
 
 # ---- d. template width -----------------------------------------------------------------------------------------------
@@ -373,7 +360,7 @@ def test_ref_template_width():
 @pytest.mark.parametrize("th", (1, 2))
 @pytest.mark.parametrize("tw", TW)
 @pytest.mark.parametrize("w", (ROW_TAPS + 1, ROW_TAPS + 2))
-def test_template_width(G, witness, w, tw, th):
+def test_template_width(lib, witness, w, tw, th):
     h = 2
     fr, tmpls = _template_inputs(w, h, tw, th)
     rw, rh = w - tw + 1, h - th + 1
@@ -384,7 +371,7 @@ def test_template_width(G, witness, w, tw, th):
         seen = set()
         for tmpl in tmpls:
             S, T, D = Region(fr.nbytes, 0, fr, 1), Region(tmpl.nbytes, 0, tmpl, 3), Region(2 * rw * rh, 0, seed=2)
-            rc, s = traced(lambda: G.gs_b200_match_template_batch(D.ptr, S.ptr, w, h, 2, T.ptr, tw, th, _stream()))
+            rc, s = traced(lambda: lib.gs_b200_match_template_batch(D.ptr, S.ptr, w, h, 2, T.ptr, tw, th, stream()))
             _ok(rc)
             got = D.read("result").reshape(2, rh, rw)
             for i in range(2):
@@ -393,7 +380,7 @@ def test_template_width(G, witness, w, tw, th):
                 assert np.array_equal(got[i], want), (i, int(tmpl.max()))
             seen |= s
         return seen
-    _witnessed(witness, "match_template-w%d-tw%d-th%d" % (w, tw, th), run, kernels)
+    witnessed(witness, run, kernels, "match_template-w%d-tw%d-th%d" % (w, tw, th))
 
 
 # ---- e. match_orb max_distance ---------------------------------------------------------------------------------------
@@ -425,12 +412,6 @@ def _match_sets():
     return [(a, b), (c, f[:0]), (e, f)]
 
 
-def _o_match(k1, k2, mm, md):
-    m = np.zeros(max(1, min(mm, len(k1))), L.MATCH_DTYPE)
-    n = O.gso_match_orb(L.ptr(k1), len(k1), L.ptr(k2 if len(k2) else np.zeros(1, L.KP_DTYPE)), len(k2), L.ptr(m), mm, md)
-    return m[:n]
-
-
 @needs_ref
 def test_ref_match_orb_extremes():
     R = L.ref()
@@ -438,15 +419,15 @@ def test_ref_match_orb_extremes():
     for md in MAX_DIST:
         for k1, k2 in sets:
             for mm in (1, len(k1) - 1, UINT_MAX):
-                want = _o_match(k1, k2, mm, md)
+                want = L.o_match(O, k1, k2, mm, md)
                 m = np.zeros(len(k1), L.MATCH_DTYPE)
                 n = R.gs_match_orb(L.ptr(k1), len(k1), L.ptr(k2 if len(k2) else np.zeros(1, L.KP_DTYPE)), len(k2),
                                    L.ptr(m), mm, md)
                 assert m[:n].tobytes() == want.tobytes(), (md, len(k1), len(k2), mm)
-    assert len(_o_match(*sets[0], UINT_MAX, 60.0)) > 10 and len(_o_match(*sets[2], UINT_MAX, 256.0)) > 0
+    assert len(L.o_match(O, *sets[0], UINT_MAX, 60.0)) > 10 and len(L.o_match(O, *sets[2], UINT_MAX, 256.0)) > 0
 
 
-def _run_match(G, sets, mm, md):
+def _run_match(lib, sets, mm, md):
     n = len(sets)
     s1, s2 = max(len(a) for a, _ in sets), max(max(len(b) for _, b in sets), 1)
     k1, k2 = np.zeros((n, s1), L.KP_DTYPE), np.zeros((n, s2), L.KP_DTYPE)
@@ -457,27 +438,27 @@ def _run_match(G, sets, mm, md):
     cap = min(mm, s1)                                    # records per pair the call can write
     K1, K2, C1, C2 = Region(k1.nbytes, 0, k1, 1), Region(k2.nbytes, 0, k2, 2), Region(4 * n, 0, c1, 3), Region(4 * n, 0, c2, 4)
     M, MC = Region(12 * n * cap, 0, seed=5), Region(4 * n, 0, seed=6)
-    rc, seen = traced(lambda: G.gs_b200_match_orb_batch(K1.ptr, C1.ptr, s1, K2.ptr, C2.ptr, s2, n, M.ptr, MC.ptr, mm, md,
-                                                       _stream()))
+    rc, seen = traced(lambda: lib.gs_b200_match_orb_batch(K1.ptr, C1.ptr, s1, K2.ptr, C2.ptr, s2, n, M.ptr, MC.ptr, mm, md,
+                                                         stream()))
     _ok(rc)
     counts, m = MC.read("counts").view(np.uint32), M.read("matches").view(L.MATCH_DTYPE).reshape(n, cap)
     for i, (a, b) in enumerate(sets):
-        want = _o_match(a, b, mm, md)
+        want = L.o_match(O, a, b, mm, md)
         assert counts[i] == len(want) and m[i, :counts[i]].tobytes() == want.tobytes(), (i, int(counts[i]), len(want))
     return seen
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("md", MAX_DIST, ids=lambda v: "md%s" % v)
-def test_match_orb_max_distance(G, witness, md):
+def test_match_orb_max_distance(lib, witness, md):
     sets = _match_sets()
 
     def run():
-        seen = _run_match(G, sets, 1, md) | _run_match(G, sets, len(sets[0][0]) - 1, md)
+        seen = _run_match(lib, sets, 1, md) | _run_match(lib, sets, len(sets[0][0]) - 1, md)
         for s in sets:     # matches hold npairs x max_matches records: UINT_MAX is one pair per call
-            seen |= _run_match(G, [s], UINT_MAX, md)
+            seen |= _run_match(lib, [s], UINT_MAX, md)
         return seen
-    _witnessed(witness, "match_orb-md%s" % md, run, ["gsb::k_match_best", "gsb::k_match_compact"])
+    witnessed(witness, run, ["gsb::k_match_best", "gsb::k_match_compact"], "match_orb-md%s" % md)
 
 
 # ---- f. radius -------------------------------------------------------------------------------------------------------
@@ -513,14 +494,14 @@ def test_ref_radius_extremes():
         for a in (rng.integers(0, 256, (h, w), dtype=np.uint8), np.full((h, w), 255, np.uint8)):
             for r in [x for x in radii(w, h) if x <= 2000] + [2000]:
                 d = np.empty_like(a); R.gs_blur(L.img(d), L.img(a), r)
-                assert np.array_equal(d, P.o_blur(O, a, r)), ("blur", w, h, r)
+                assert np.array_equal(d, L.o_blur(O, a, r)), ("blur", w, h, r)
                 d = np.empty_like(a); R.gs_adaptive_threshold(L.img(d), L.img(a), r, -3)
-                assert np.array_equal(d, P.o_adaptive(O, a, r, -3)), ("adaptive", w, h, r)
+                assert np.array_equal(d, L.o_adaptive(O, a, r, -3)), ("adaptive", w, h, r)
     for w, h in TINY + MEDIUM:
         a = L.natural_like(w, h, 4)
-        full_b, full_a = P.o_blur(O, a, max(w, h)), P.o_adaptive(O, a, max(w, h), -3)
+        full_b, full_a = L.o_blur(O, a, max(w, h)), L.o_adaptive(O, a, max(w, h), -3)
         for r in (max(w, h) - 1, 4096, 65535, INT_MAX):
-            assert np.array_equal(P.o_blur(O, a, r), full_b) and np.array_equal(P.o_adaptive(O, a, r, -3), full_a), r
+            assert np.array_equal(L.o_blur(O, a, r), full_b) and np.array_equal(L.o_adaptive(O, a, r, -3), full_a), r
 
 
 def _radius_cases():
@@ -530,23 +511,23 @@ def _radius_cases():
 @pytest.mark.gpu
 @pytest.mark.parametrize("w,h,r,op", [pytest.param(*c, id="%s-%dx%d-r%d" % (c[3], c[0], c[1], c[2]))
                                       for c in _radius_cases()])
-def test_radius_extremes(G, witness, w, h, r, op):
+def test_radius_extremes(lib, witness, w, h, r, op):
     adaptive, c = op == "adaptive", -3
     fr = frames(w, h, 3, w + h)
 
     def run():
         S, D = Region(fr.nbytes, 0, fr, 1), Region(fr.nbytes, 0, seed=2)
         if adaptive:
-            rc, seen = traced(lambda: G.gs_b200_adaptive_threshold_batch(D.ptr, S.ptr, w, h, 3, r, c, _stream()))
+            rc, seen = traced(lambda: lib.gs_b200_adaptive_threshold_batch(D.ptr, S.ptr, w, h, 3, r, c, stream()))
         else:
-            rc, seen = traced(lambda: G.gs_b200_blur_batch(D.ptr, S.ptr, w, h, 3, r, _stream()))
+            rc, seen = traced(lambda: lib.gs_b200_blur_batch(D.ptr, S.ptr, w, h, 3, r, stream()))
         _ok(rc)
         got = D.read("dst").reshape(3, h, w)
         for i in range(3):
-            want = P.o_adaptive(O, fr[i], r, c) if adaptive else P.o_blur(O, fr[i], r)
+            want = L.o_adaptive(O, fr[i], r, c) if adaptive else L.o_blur(O, fr[i], r)
             assert np.array_equal(got[i], want), i
         return seen
-    _witnessed(witness, "%s-%dx%d-r%d" % (op, w, h, r), run, [box_route(w, r, adaptive, c)])
+    witnessed(witness, run, [box_route(w, r, adaptive, c)], "%s-%dx%d-r%d" % (op, w, h, r))
 
 
 # ---- g. integral wrap, LBP on the wrapped table ----------------------------------------------------------------------
@@ -579,7 +560,7 @@ def test_ref_integral_wrap():
     R = L.ref()
     f = wrap_frame()
     ii = np.empty(f.shape, np.uint32); R.gs_integral(L.img(f), L.ptr(ii))
-    assert np.array_equal(ii, P.o_integral(O, f))
+    assert np.array_equal(ii, L.o_integral(O, f))
     assert int(ii[-1, -1]) == int(f.sum(dtype=np.uint64)) % 2 ** 32 and int(f.sum(dtype=np.uint64)) >= 2 ** 32
 
 
@@ -590,22 +571,22 @@ def test_ref_lbp_on_wrapped_table():
     first row and column"""
     R = L.ref()
     lena = np.load(os.path.join(L.ROOT, "tests", "golden", "lena_golden.npz"))["lena"]
-    ii = P.o_integral(O, np.ascontiguousarray(lena))
+    ii = L.o_integral(O, np.ascontiguousarray(lena))
     wrapped = ((ii.astype(np.uint64) + 2 ** 32 - 4096) % 2 ** 32).astype(np.uint32)
     assert (wrapped < ii).mean() > 0.9
     cas = L.HostCascade()
     for t in (ii, wrapped):
-        want = P.o_detect(O, cas, t, 1000, 1.1, 1.0, 4.0, 1)
+        want = L.o_detect(O, cas, t, 1000, 1.1, 1.0, 4.0, 1)
         r = np.zeros(1000, L.RECT_DTYPE)
         n = R.gs_lbp_detect(cas.ptr, L.ptr(t), 128, 128, L.ptr(r), 1000, 1.1, 1.0, 4.0, 1)
         assert r[:n].tobytes() == want.tobytes() and n > 0
 
 
 @pytest.mark.gpu
-def test_integral_wrap_and_lbp(G, witness):
+def test_integral_wrap_and_lbp(lib, witness):
     import torch
     frs = [wrap_frame(0), wrap_frame(1)]
-    want = [torch.from_numpy(P.o_integral(O, f).view(np.int32)).cuda() for f in frs]
+    want = [torch.from_numpy(L.o_integral(O, f).view(np.int32)).cuda() for f in frs]
     px = WRAP_W * WRAP_W
 
     def integral(env, n, ii_off):
@@ -615,7 +596,7 @@ def test_integral_wrap_and_lbp(G, witness):
         if env:
             os.environ["GS_B200_INTEGRAL"] = env
         try:
-            rc, seen = traced(lambda: G.gs_b200_integral_batch(ptr, src.data_ptr(), WRAP_W, WRAP_W, n, _stream()))
+            rc, seen = traced(lambda: lib.gs_b200_integral_batch(ptr, src.data_ptr(), WRAP_W, WRAP_W, n, stream()))
         finally:
             os.environ.pop("GS_B200_INTEGRAL", None)
         _ok(rc)
@@ -629,27 +610,27 @@ def test_integral_wrap_and_lbp(G, witness):
     rows_cols = ["gsb::k_integral_rows<false>", "gsb::k_integral_cols"]
     for env, n, off, kernels in (("strips", 1, 0, ["gsb::k_integral_strips<128, 8>"]),
                                  ("bands", 32, 0, ["gsb::k_integral_bands<1024>"]), (None, 1, 4, rows_cols)):
-        _witnessed(witness, "integral-%s-%dx%d-n%d-ii%d" % (env or "rows_cols", WRAP_W, WRAP_W, n, off),
-                   lambda: integral(env, n, off)[0], kernels)
+        witnessed(witness, lambda: integral(env, n, off)[0], kernels,
+                  "integral-%s-%dx%d-n%d-ii%d" % (env or "rows_cols", WRAP_W, WRAP_W, n, off))
 
     _, tables = integral("strips", 1, 0)
     cas = L.HostCascade()
     sf, mn, mx, step = WRAP_LBP
     mr = 1000
-    ref_rects = P.o_detect(O, cas, want[0].cpu().numpy().view(np.uint32), mr, sf, mn, mx, step)
+    ref_rects = L.o_detect(O, cas, want[0].cpu().numpy().view(np.uint32), mr, sf, mn, mx, step)
     _assert_wrapped(frs[0], ref_rects)
 
     def lbp():
         RR = torch.zeros(mr * 4, dtype=torch.int32, device="cuda")
         N = torch.zeros(1, dtype=torch.int32, device="cuda")
-        rc, seen = traced(lambda: G.gs_b200_lbp_detect_batch(cas.ptr, tables.data_ptr(), WRAP_W, WRAP_W, 1, RR.data_ptr(),
-                                                             N.data_ptr(), mr, sf, mn, mx, step, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_lbp_detect_batch(cas.ptr, tables.data_ptr(), WRAP_W, WRAP_W, 1, RR.data_ptr(),
+                                                               N.data_ptr(), mr, sf, mn, mx, step, stream()))
         _ok(rc)
         n = int(N.item())
         got = RR.cpu().numpy().view(np.uint32).reshape(mr, 4)[:n]
         assert got.tobytes() == ref_rects.tobytes(), (n, len(ref_rects))
         return seen
-    _witnessed(witness, "lbp-on-wrapped-table", lbp, ["gsb::k_lbp_emit"])
+    witnessed(witness, lbp, ["gsb::k_lbp_emit"], "lbp-on-wrapped-table")
 
 
 # ---- h. ORB nkps -----------------------------------------------------------------------------------------------------
@@ -662,7 +643,7 @@ def _orb_frame():
 
 
 def _fast_survivors(a):
-    return len(P.o_fast(O, a, np.zeros_like(a), 10 ** 6, 20))
+    return len(L.o_fast(O, a, np.zeros_like(a), 10 ** 6, 20))
 
 
 @needs_ref
@@ -674,27 +655,27 @@ def test_ref_orb_nkps():
     for nk in NKPS:
         kr = np.zeros(nk, L.KP_DTYPE)
         n = R.gs_orb_extract(L.img(a), L.ptr(kr), nk, 20, L.ptr(np.zeros_like(a)))
-        ko = P.o_orb(O, a, np.zeros_like(a), nk, 20)
+        ko = L.o_orb(O, a, np.zeros_like(a), nk, 20)
         assert n == len(ko) and kr[:n].tobytes() == ko.tobytes(), nk
         assert n == (0 if nk == 1 else nk), (nk, n)    # nkps = 1: the 4 candidates all lie in the 15-px margin
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("nk", NKPS)
-def test_orb_nkps(G, witness, nk):
+def test_orb_nkps(lib, witness, nk):
     a = _orb_frame()
     h, w = a.shape
 
     def run():
         S, SM = Region(a.nbytes, 0, a, 1), Region(a.nbytes, 0, np.zeros_like(a), 4)
         K, N = Region(48 * nk, 0, seed=5), Region(4, 0, seed=6)
-        rc, seen = traced(lambda: G.gs_b200_orb_extract_batch(S.ptr, w, h, 1, SM.ptr, K.ptr, N.ptr, nk, 20, _stream()))
+        rc, seen = traced(lambda: lib.gs_b200_orb_extract_batch(S.ptr, w, h, 1, SM.ptr, K.ptr, N.ptr, nk, 20, stream()))
         _ok(rc)
         cnt = int(N.read("counts").view(np.uint32)[0])
         got = K.read("kps").view(L.KP_DTYPE)[:cnt]
         sm = np.zeros_like(a)
-        want = P.o_orb(O, a, sm, nk, 20)
+        want = L.o_orb(O, a, sm, nk, 20)
         assert cnt == len(want) == (0 if nk == 1 else nk) and got.tobytes() == want.tobytes(), (cnt, len(want))
         assert np.array_equal(SM.read("scoremap").reshape(h, w), sm)
         return seen
-    _witnessed(witness, "orb-1920x1080-nkps%d" % nk, run, ["gsb::k_orb_select", "gsb::k_orb_brief<true>"])
+    witnessed(witness, run, ["gsb::k_orb_select", "gsb::k_orb_brief<true>"], "orb-1920x1080-nkps%d" % nk)
