@@ -428,7 +428,7 @@ int gs_b200_blobs_batch(const uint8_t *img, unsigned w, unsigned h, unsigned n, 
   const size_t ws_a = 3 * words_b + sizeof(unsigned) * (rows_total + n) + 7 * sizeof(unsigned) * (size_t)nblobs * n;
   unsigned *wa = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_BLOB_A, ws_a));
   unsigned *parent = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_BLOB_B, sizeof(unsigned) * (size_t)w * h * n));
-  if (!wa || !parent) return (int)cudaErrorMemoryAllocation;
+  if (!wa || !parent) return gsb::workspace_error();
   unsigned *mask = wa, *seed = wa + words_total, *sprefix = seed + words_total, *rowoff = sprefix + words_total;
   unsigned *totals = rowoff + rows_total, *stats = totals + n;
   const size_t sn = (size_t)nblobs * n;

@@ -1163,7 +1163,7 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
   }
   // other radii / ragged widths: the two per-op kernels through a scratch frame batch (same result, 4 B/px)
   uint8_t *tmp = static_cast<uint8_t *>(gsb::workspace(s, gsb::WS_STAGE_FUSED, (size_t)w * h * n));
-  if (!tmp) return (int)cudaErrorMemoryAllocation;
+  if (!tmp) return gsb::workspace_error();
   int rc = gs_b200_blur_batch(tmp, src, w, h, n, radius, st);
   if (rc) return rc;
   return gs_b200_sobel_batch(dst, tmp, w, h, n, st);

@@ -57,9 +57,18 @@ int launch(const char *file, int line, void (*k)(P...), dim3 grid, dim3 block, s
     }                                                   \
   } while (0)
 
-// Grow-only device scratch, one arena per (device, stream, slot).  Not freed until process
-// exit: the hot path must not cudaMalloc per call.  Returns nullptr on allocation failure.
+// Grow-only device scratch, one arena per (device, stream, slot); cudaStreamPerThread has one per (host thread, device,
+// slot), freed at thread exit.  Not freed until process exit otherwise: the hot path must not cudaMalloc per call.
+// Returns nullptr when it cannot allocate, or when it would have to grow while `s` is capturing a graph;
+// workspace_error() is then the calling thread's error code (its text is in gs_b200_last_error()).
 void *workspace(cudaStream_t s, int slot, size_t bytes);
+int workspace_error();
+// whether `s` is capturing a CUDA graph (true also when the query itself is not legal in the current capture)
+bool capturing(cudaStream_t s);
+// Blocking host -> device copy that no caller's stream can overtake: a copy on a private non-blocking stream, then a
+// sync of that stream.  (A pageable cudaMemcpy on the legacy stream may return before its DMA lands, and kernels on
+// non-blocking streams are not ordered after it.)  For rare uploads only: LBP plan misses, once-per-device tables.
+int upload(void *dst, const void *src, size_t bytes, const char *file, int line);
 
 enum { WS_INTEGRAL = 0, WS_FAST_A, WS_FAST_B, WS_ORB_A, WS_ORB_B, WS_LBP_A, WS_LBP_B, WS_LBP_C,
        WS_STAGE_A, WS_STAGE_B, WS_STAGE_C, WS_STAGE_D, WS_HIST, WS_STAGE_FUSED, WS_BLOB_A, WS_BLOB_B, WS_BLOB_C, WS_MORPH, WS_SLOTS };

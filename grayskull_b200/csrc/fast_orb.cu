@@ -40,27 +40,31 @@ __device__ const uint32_t c_brief[256] = {
 };
 
 // the same offsets as floats (x1, y1, x2, y2): k_orb_brief converts nothing on the conversion pipe (four I2F per lane and
-// pattern word ran at 16 lanes/clk/SM next to the four float->int truncations).  Filled once per device by k_brief_init.
+// pattern word ran at 16 lanes/clk/SM next to the four float->int truncations).  Filled once per device by
+// brief_table_init.
 __device__ float4 c_brieff[256];
 static const uint32_t h_brief[256] = {
 #include "brief_pattern.inc"
 };
-// once per device, synchronous (cudaMemcpyToSymbol from pageable memory returns after the copy): no stream can see a
-// half-filled table
-static int brief_table_init() {
+// once per device, by upload(): the copy has landed before the first k_orb_brief is enqueued on any stream, so no
+// stream can see a half-filled table.  The first ORB call on a device must not be captured into a graph.
+static int brief_table_init(cudaStream_t user) {
   static std::mutex mu;
   static bool filled[64];
   int dev = 0;
   GSB_CHECK(cudaGetDevice(&dev));
   std::lock_guard<std::mutex> lock(mu);
   if (filled[dev & 63]) return 0;
+  if (capturing(user)) return record_error(cudaErrorStreamCaptureUnsupported, __FILE__, __LINE__);
   float4 t[256];
   for (int i = 0; i < 256; i++) {
     const uint32_t pk = h_brief[i];
     t[i] = make_float4((float)(int)(int8_t)(pk & 0xFF), (float)(int)(int8_t)((pk >> 8) & 0xFF),
                        (float)(int)(int8_t)((pk >> 16) & 0xFF), (float)(int)(int8_t)(pk >> 24));
   }
-  GSB_CHECK(cudaMemcpyToSymbol(c_brieff, t, sizeof(t)));
+  void *sym = nullptr;
+  GSB_CHECK(cudaGetSymbolAddress(&sym, c_brieff));
+  if (int rc = upload(sym, t, sizeof(t), __FILE__, __LINE__)) return rc;
   filled[dev & 63] = true;
   return 0;
 }
@@ -941,7 +945,7 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
   const unsigned rows = h - 6, mw = (w + 31) / 32;
   unsigned *rowcount = static_cast<unsigned *>(workspace(s, WS_FAST_A, sizeof(unsigned) * (size_t)rows * n));
   unsigned *masks = static_cast<unsigned *>(workspace(s, WS_FAST_B, sizeof(unsigned) * (size_t)rows * n * mw));
-  if (!rowcount || !masks) return (int)cudaErrorMemoryAllocation;
+  if (!rowcount || !masks) return gsb::workspace_error();
   GSB_ASSERT(n <= 65535u && rows <= 0x7FFFFFFFu);
   // thresholds above 255 (the reference computes p + t / p - t in unsigned arithmetic, :496-498, which wraps for
   // huge t) take the literal per-pixel kernel: the tiled kernel's 16-bit lane arithmetic assumes t <= 255
@@ -1001,7 +1005,7 @@ int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsign
   const unsigned cap = nkps * 4ull < gsb::ORB_MAXC ? nkps * 4 : gsb::ORB_MAXC;  // reference :656
   gsb::KpRec *cand = static_cast<gsb::KpRec *>(gsb::workspace(st, gsb::WS_ORB_A, sizeof(gsb::KpRec) * (size_t)cap * n));
   unsigned *ccount = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_ORB_B, sizeof(unsigned) * n));
-  if (!cand || !ccount) return (int)cudaErrorMemoryAllocation;
+  if (!cand || !ccount) return gsb::workspace_error();
   int rc = gsb::fast_impl(src, w, h, n, scoremap, w, h, cand, ccount, cap, threshold, st);
   if (rc) return rc;
   GSB_LAUNCH(gsb::k_orb_select, n, 256, 0, st, cand, ccount, cap, w, h, reinterpret_cast<gsb::KpRec *>(kps), counts, nkps);
@@ -1012,7 +1016,7 @@ int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsign
   if (gsb::g_trig_mode == 0) gsb::trig_selfcheck_once(st);
   GSB_LAUNCH(gsb::k_orb_moments, (unsigned)blocks, 256, 0, st, src, w, h, kr, counts, nkps, n);
   GSB_LAUNCH(gsb::k_orb_trig, (unsigned)((warps + 255) / 256), 256, 0, st, kr, counts, nkps, n, gsb::g_trig_mode);
-  if (int rcb = gsb::brief_table_init()) return rcb;
+  if (int rcb = gsb::brief_table_init(st)) return rcb;
   const bool words = w % 4 == 0 && reinterpret_cast<uintptr_t>(src) % 4 == 0 && !gsb::force_generic();
   GSB_LAUNCH(words ? gsb::k_orb_brief<true> : gsb::k_orb_brief<false>, (unsigned)blocks, 256, 0, st, src, w, h, kr, counts, nkps,
              n);

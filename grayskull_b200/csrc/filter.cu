@@ -271,8 +271,14 @@ int gs_b200_filter_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned 
     }
   }
   const size_t kbytes = has_kernel ? (size_t)kw * kh : 0;
+  // The weights go to the device by a copy from the caller's (pageable) host memory.  A graph would capture the host
+  // pointer, not the values, so this path refuses capture; the 3x3 path above passes its weights by value.
+  if (kbytes && gsb::capturing(st)) {
+    gsb::record_error(cudaErrorStreamCaptureUnsupported, __FILE__, __LINE__);
+    return (int)cudaErrorStreamCaptureUnsupported;
+  }
   int8_t *dk = static_cast<int8_t *>(gsb::workspace(st, gsb::WS_HIST, kbytes + 16));
-  if (!dk) return (int)cudaErrorMemoryAllocation;
+  if (!dk) return gsb::workspace_error();
   if (kbytes) GSB_CHECK(cudaMemcpyAsync(dk, kernel, kbytes, cudaMemcpyHostToDevice, st));
   dim3 grid((w + 31) / 32, (h + 7) / 8, zn);
   GSB_ASSERT(grid.y <= 65535u);
@@ -291,7 +297,7 @@ int gs_b200_match_template_batch(uint8_t *result, const uint8_t *img, unsigned w
   if (w % 4 == 0 && reinterpret_cast<uintptr_t>(img) % 4 == 0 && tw < 66051u) {
     const unsigned twords = (tw + 3) / 4;
     uint32_t *tpack = static_cast<uint32_t *>(gsb::workspace(st, gsb::WS_HIST, sizeof(uint32_t) * (size_t)twords * th));
-    if (!tpack) return (int)cudaErrorMemoryAllocation;
+    if (!tpack) return gsb::workspace_error();
     GSB_LAUNCH(gsb::k_pack_template, (twords * th + 255) / 256, 256, 0, st, tpack, tmpl, tw, th, twords);
     dim3 grid(((rw + 3) / 4 + 31) / 32, (rh + 7) / 8, zn);
     GSB_ASSERT(grid.y <= 65535u);
@@ -313,7 +319,7 @@ int gs_b200_find_best_match_batch(struct gs_point *best, const uint8_t *result, 
   GSB_ASSERT(n <= 65535u);
   const size_t px = (size_t)rw * rh;
   unsigned long long *keys = static_cast<unsigned long long *>(gsb::workspace(st, gsb::WS_HIST, sizeof(unsigned long long) * n));
-  if (!keys) return (int)cudaErrorMemoryAllocation;
+  if (!keys) return gsb::workspace_error();
   GSB_CHECK(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * n, st));
   dim3 grid((unsigned)((px + gsb::BM_CHUNK - 1) / gsb::BM_CHUNK), n);
   GSB_LAUNCH(gsb::k_best_match_partial, grid, 256, 0, st, keys, result, px);

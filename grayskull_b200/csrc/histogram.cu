@@ -223,7 +223,7 @@ int gs_b200_otsu_threshold_batch(uint8_t *thresh, unsigned *hist, const uint8_t 
   cudaStream_t st = static_cast<cudaStream_t>(s);
   if (!hist) {
     hist = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_HIST, sizeof(unsigned) * 256 * (size_t)n));
-    if (!hist) return (int)cudaErrorMemoryAllocation;
+    if (!hist) return gsb::workspace_error();
   }
   int rc = gs_b200_histogram_batch(hist, src, w, h, n, s);
   if (rc) return rc;

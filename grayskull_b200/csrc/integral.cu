@@ -324,7 +324,7 @@ extern "C" int gs_b200_integral_batch(uint32_t *ii, const uint8_t *src, unsigned
     if (want && !(env && env[0] == 'b') && w % 8 == 0 && strips <= 16 && aligned && !gsb::force_generic() && ctas < 0x7FFFFFFFull) {
       const size_t slot_bytes = sizeof(unsigned long long) * (size_t)ctas * nbands * rb;
       unsigned char *ws = static_cast<unsigned char *>(gsb::workspace(st, gsb::WS_INTEGRAL, 256 + slot_bytes));
-      if (!ws) return (int)cudaErrorMemoryAllocation;
+      if (!ws) return gsb::workspace_error();
       GSB_CHECK(cudaMemsetAsync(ws, 0, 256 + (strips > 1 ? slot_bytes : 0), st));
       GSB_LAUNCH(narrow ? gsb::k_integral_strips<64, 16> : gsb::k_integral_strips<128, 8>, (unsigned)ctas, narrow ? 64 : 128, 0,
                  st, ii, src, w, h, n, strips, nbands, reinterpret_cast<unsigned *>(ws),
@@ -337,7 +337,7 @@ extern "C" int gs_b200_integral_batch(uint32_t *ii, const uint8_t *src, unsigned
     const unsigned nbands = (h + gsb::IB_BH - 1) / gsb::IB_BH;
     const size_t ctrl_bytes = sizeof(unsigned) * (1 + (size_t)n * nbands);
     unsigned *ctrl = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_INTEGRAL, ctrl_bytes));
-    if (!ctrl) return (int)cudaErrorMemoryAllocation;
+    if (!ctrl) return gsb::workspace_error();
     GSB_CHECK(cudaMemsetAsync(ctrl, 0, ctrl_bytes, st));
     const unsigned threads = ((w / 8 + 31) / 32) * 32;
     const size_t smem = sizeof(uint32_t) * gsb::IB_BH * threads;   // <= 64 KB

@@ -718,8 +718,9 @@ static void build_scales(const struct gs_lbp_cascade *c, unsigned iw, unsigned i
   }
 }
 
+// the cached plan of this cascade and geometry; on a miss it is built and uploaded (blocking) unless !may_build
 static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih, float sf, float mn, float mx,
-                        int step) {
+                        int step, bool may_build) {
   int dev = 0;
   cudaGetDevice(&dev);
   // test hook: 1 = every scale on the 1024-thread tile form, 0 = none, unset = by tile height (tests reach both
@@ -729,6 +730,7 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
   std::lock_guard<std::mutex> lock(g_plan_mutex);
   for (auto &r : g_plans)
     if (r->key == key) return r;
+  if (!may_build) return nullptr;
 
   PlanRef ref = std::make_shared<PlanEntry>();
   PlanEntry &e = *ref;
@@ -853,7 +855,7 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
   memcpy(&host[o_st], stages.data(), sizeof(Stage) * nst);
   if (!geo.empty()) memcpy(&host[o_ge], geo.data(), sizeof(FeatGeo) * geo.size());
   if (cudaMalloc(&e.blob, total) != cudaSuccess) return nullptr;
-  if (cudaMemcpy(e.blob, host.data(), total, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+  if (upload(e.blob, host.data(), total, __FILE__, __LINE__)) return nullptr;
   unsigned char *b = static_cast<unsigned char *>(e.blob);
   e.dc.scales = reinterpret_cast<const ScaleInfo *>(b + o_sc);
   e.dc.feat = reinterpret_cast<const short4 *>(b + o_ft);
@@ -907,8 +909,10 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
   GSB_ASSERT(rects || max_rects == 0);
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(s);
-  gsb::PlanRef p = gsb::get_plan(c, iw, ih, scale_factor, min_scale, max_scale, step);
-  if (!p) return gsb::record_error(cudaErrorMemoryAllocation, __FILE__, __LINE__);
+  // a plan miss allocates and uploads synchronously, which a graph capture cannot hold
+  const bool cap = gsb::capturing(st);
+  gsb::PlanRef p = gsb::get_plan(c, iw, ih, scale_factor, min_scale, max_scale, step, !cap);
+  if (!p) return gsb::record_error(cap ? cudaErrorStreamCaptureUnsupported : cudaErrorMemoryAllocation, __FILE__, __LINE__);
   const gsb::DevCascade &dc = p->dc;
   if (dc.total_slots == 0 || max_rects == 0) {
     GSB_CHECK(cudaMemsetAsync(counts, 0, sizeof(unsigned) * n, st));
@@ -918,7 +922,7 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
   GSB_ASSERT(nblocks < 0x7FFFFFFFull && n <= 65535u);
   unsigned *masks = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_LBP_A, 4 * (size_t)dc.total_slots * n));
   unsigned *bcount = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_LBP_B, 4 * (size_t)nblocks * n));
-  if (!masks || !bcount) return (int)cudaErrorMemoryAllocation;
+  if (!masks || !bcount) return gsb::workspace_error();
   dim3 grid((unsigned)nblocks, n);
   const size_t table_bytes = sizeof(gsb::FeatGeo) * dc.nfeatures + sizeof(gsb::Weak) * dc.nweaks +
                              sizeof(gsb::Stage) * dc.nstages + 4 * (size_t)dc.nsubsets;
@@ -935,7 +939,7 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
     if (const char *ce = getenv("GS_B200_LBP_CHUNK_FRAMES")) chunk = (unsigned)atoi(ce);   // test hook
     chunk = chunk < 1 ? 1 : (chunk > n ? n : chunk);
     uint32_t *planes = static_cast<uint32_t *>(gsb::workspace(st, gsb::WS_LBP_C, frame_bytes * chunk));
-    if (!planes) return (int)cudaErrorMemoryAllocation;
+    if (!planes) return gsb::workspace_error();
     for (unsigned f0 = 0; f0 < n; f0 += chunk) {
       const unsigned nf = n - f0 < chunk ? n - f0 : chunk;
       const uint32_t *src = ii + (size_t)f0 * iw * ih;
@@ -992,7 +996,7 @@ int gsb_lbp_window_single(const struct gs_lbp_cascade *c, const uint32_t *ii, un
   const size_t o_sb = (o_wk + sizeof(gsb::Weak) * nw + 15) & ~(size_t)15;
   const size_t o_st = (o_sb + 4 * (size_t)nsub + 15) & ~(size_t)15, total = o_st + sizeof(gsb::Stage) * nst;
   unsigned char *blob = static_cast<unsigned char *>(gsb::workspace(s, gsb::WS_LBP_C, total));
-  if (!blob) return (int)cudaErrorMemoryAllocation;
+  if (!blob) return gsb::workspace_error();
   GSB_CHECK(cudaMemcpyAsync(blob + o_ft, feat.data(), sizeof(short4) * nf, cudaMemcpyHostToDevice, s));
   GSB_CHECK(cudaMemcpyAsync(blob + o_wk, weaks.data(), sizeof(gsb::Weak) * nw, cudaMemcpyHostToDevice, s));
   GSB_CHECK(cudaMemcpyAsync(blob + o_sb, c->subsets, 4 * (size_t)nsub, cudaMemcpyHostToDevice, s));

@@ -167,7 +167,7 @@ extern "C" int gs_b200_match_orb_batch(const struct gs_keypoint *kps1, const uns
   }
   GSB_ASSERT(npairs <= 65535u && stride1 < 0x7FFFFFFFu && stride2 < (1u << gsb::MT_IDX_BITS));
   uint2 *cand = static_cast<uint2 *>(gsb::workspace(st, gsb::WS_ORB_A, sizeof(uint2) * (size_t)stride1 * npairs));
-  if (!cand) return (int)cudaErrorMemoryAllocation;
+  if (!cand) return gsb::workspace_error();
   GSB_LAUNCH(gsb::k_match_best, dim3((stride1 + gsb::MT_QPC - 1) / gsb::MT_QPC, npairs), 256, 0, st,
              reinterpret_cast<const gsb::KpRec48 *>(kps1), n1, stride1, reinterpret_cast<const gsb::KpRec48 *>(kps2), n2, stride2,
              max_distance, cand);

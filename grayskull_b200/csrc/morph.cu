@@ -338,7 +338,7 @@ static int launch_morph_n(uint8_t *dst, const uint8_t *src, unsigned w, unsigned
   // are N+M passes), ceil(N/16) launches of 2 B/px, which beats the row / column passes up to N = 48 (DESIGN.md §6)
   if (ne <= MT_COMPOSE_MAX && tma) {
     uint8_t *ws = static_cast<uint8_t *>(workspace(s, WS_MORPH, chunk * fb));
-    if (!ws) return static_cast<int>(cudaErrorMemoryAllocation);
+    if (!ws) return gsb::workspace_error();
     const unsigned steps = (ne + MT_MAX_N - 1) / MT_MAX_N;
     for (size_t f0 = 0; f0 < n; f0 += chunk) {
       const unsigned c = (unsigned)(n - f0 < chunk ? n - f0 : chunk);
@@ -360,7 +360,7 @@ static int launch_morph_n(uint8_t *dst, const uint8_t *src, unsigned w, unsigned
   }
   // path B: row pass into the workspace, column pass into dst
   uint8_t *ws = static_cast<uint8_t *>(workspace(s, WS_MORPH, chunk * fb));
-  if (!ws) return static_cast<int>(cudaErrorMemoryAllocation);
+  if (!ws) return gsb::workspace_error();
   for (size_t f0 = 0; f0 < n; f0 += chunk) {
     const size_t c = n - f0 < chunk ? n - f0 : chunk;
     const unsigned long long rows = (unsigned long long)c * h, cols = (unsigned long long)c * w;

@@ -71,12 +71,61 @@ struct Arena {
 static std::mutex g_ws_mutex;
 static std::map<std::tuple<int, cudaStream_t, int>, Arena> g_ws;
 
+// cudaStreamPerThread is one handle for a different stream in each host thread, so its arenas cannot be keyed by the
+// handle: each thread keeps its own, and frees them at thread exit once that thread's stream has drained.
+struct ThreadArenas {
+  std::map<std::pair<int, int>, Arena> m;   // (device, slot)
+  ~ThreadArenas() {
+    int cur = 0;
+    if (cudaGetDevice(&cur) != cudaSuccess) return;   // runtime already shut down
+    for (auto &kv : m) {
+      if (!kv.second.ptr) continue;
+      if (cudaSetDevice(kv.first.first) != cudaSuccess) continue;
+      cudaStreamSynchronize(cudaStreamPerThread);
+      cudaFree(kv.second.ptr);
+    }
+    cudaSetDevice(cur);
+  }
+};
+static thread_local ThreadArenas t_ws;
+static thread_local int t_ws_error = cudaErrorMemoryAllocation;
+
+bool capturing(cudaStream_t s) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(s, &cs) != cudaSuccess) {
+    cudaGetLastError();
+    return true;   // e.g. the legacy stream while another stream captures: no allocation or sync is legal either
+  }
+  return cs != cudaStreamCaptureStatusNone;
+}
+
+int workspace_error() { return t_ws_error; }
+
+int upload(void *dst, const void *src, size_t bytes, const char *file, int line) {
+  cudaStream_t st = nullptr;
+  cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (st) cudaStreamDestroy(st);
+  return e == cudaSuccess ? 0 : record_error(e, file, line);
+}
+
 void *workspace(cudaStream_t s, int slot, size_t bytes) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  std::lock_guard<std::mutex> lock(g_ws_mutex);
-  Arena &a = g_ws[std::make_tuple(dev, s, slot)];
+  const bool per_thread = s == cudaStreamPerThread;
+  std::unique_lock<std::mutex> lock(g_ws_mutex, std::defer_lock);
+  if (!per_thread) lock.lock();
+  Arena &a = per_thread ? t_ws.m[std::make_pair(dev, slot)] : g_ws[std::make_tuple(dev, s, slot)];
   if (a.bytes >= bytes && a.ptr) return a.ptr;
+  if (capturing(s)) {
+    // growing would synchronise, free and allocate inside the capture; the arena stays as it is
+    t_ws_error = record_error(cudaErrorStreamCaptureUnsupported, __FILE__, __LINE__);
+    snprintf(t_last_error, sizeof(t_last_error),
+             "cudaErrorStreamCaptureUnsupported: workspace slot %d must grow to %zu bytes while the stream is capturing; "
+             "run the call once at this geometry on this stream before capturing it", slot, bytes);
+    return nullptr;
+  }
   if (a.ptr) {
     // the old arena may still be in use by work queued on `s`
     cudaStreamSynchronize(s);
@@ -86,7 +135,7 @@ void *workspace(cudaStream_t s, int slot, size_t bytes) {
   size_t want = bytes + bytes / 4 + 256;
   if (cudaMalloc(&a.ptr, want) != cudaSuccess) {
     a.ptr = nullptr;
-    record_error(cudaGetLastError(), __FILE__, __LINE__);
+    t_ws_error = record_error(cudaGetLastError(), __FILE__, __LINE__);
     return nullptr;
   }
   a.bytes = want;
