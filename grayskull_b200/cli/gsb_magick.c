@@ -10,6 +10,7 @@
  *   blur:R   sobel   erode[:N]   dilate[:N]   adaptive:R:C   threshold:T   threshold:otsu[+K]
  *   (erode:N / dilate:N are N passes of the 3x3 op in one call, gs_b200_erode_n_batch / gs_b200_dilate_n_batch)
  *   filter:sharpen|emboss|box|gaussian   downsample   resize:W:H
+ *   crop:X:Y:W:H    (the reference's crop verb, nanomagick.c:69-77: gs_crop of one rectangle of every frame)
  *   keypoints:N:T   (prints the ORB keypoint count per frame; frames pass through unchanged)
  *   blobs:N         (prints the number of 4-connected components >= 128 per frame; frames pass through unchanged)
  *   scan:W:H        (the reference's document scanner, nanomagick.c:186-210, per frame on the device: blur 1 ->
@@ -19,7 +20,7 @@
  */
 #include <string.h>
 
-#include "grayskull_b200.h"
+#include "grayskull_b200_roi.h"
 
 #define DIE(...) (fprintf(stderr, "gsb_magick: " __VA_ARGS__), fprintf(stderr, "\n"), exit(1))
 #define CK(call)                                                         \
@@ -98,6 +99,16 @@ static void stage(const char *spec, struct batch *cur, struct batch *tmp, size_t
     if (dw <= 0 || dh <= 0) DIE("bad size in '%s'", spec);
     ensure(tmp, (unsigned)dw, (unsigned)dh, n, cap_tmp);
     CK(gs_b200_resize_batch(tmp->dev, (unsigned)dw, (unsigned)dh, cur->dev, w, h, n, NULL));
+  } else if (!strcmp(name, "crop")) {
+    int x, y, cw, ch;
+    char extra;
+    struct gs_rect roi;
+    if (sscanf(spec, "crop:%d:%d:%d:%d%c", &x, &y, &cw, &ch, &extra) != 4) DIE("bad rectangle in '%s' (crop:X:Y:W:H)", spec);
+    if (x < 0 || y < 0 || cw <= 0 || ch <= 0 || (long)x + cw > (long)w || (long)y + ch > (long)h)
+      DIE("invalid crop rectangle in '%s' for %ux%u frames", spec, w, h);
+    roi.x = (unsigned)x, roi.y = (unsigned)y, roi.w = (unsigned)cw, roi.h = (unsigned)ch;
+    ensure(tmp, roi.w, roi.h, n, cap_tmp);
+    CK(gs_b200_crop_resize_batch(tmp->dev, roi.w, roi.h, cur->dev, w, h, n, roi, GS_B200_NEAREST, NULL));
   } else if (!strcmp(name, "keypoints") && nargs == 2) {
     unsigned nk = (unsigned)atoi(a0), f, *counts, *hc;
     struct gs_keypoint *kps;

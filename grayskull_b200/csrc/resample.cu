@@ -1,5 +1,6 @@
 // resample.cu -- gs_resize and gs_downsample (reference grayskull.h:171-197).
 #include "common.cuh"
+#include "resample.cuh"
 
 namespace gsb {
 
@@ -38,20 +39,7 @@ __global__ void k_downsample_generic(uint8_t *__restrict__ dst, const uint8_t *_
 }
 
 // ---- gs_resize: pixel-centre bilinear, fp32 in the reference's exact evaluation order ---------
-// Every rounding step of grayskull.h:174-184 is reproduced with the _rn intrinsics (never
-// contracted into FMAs): sx = ((x + 0.5f) * sw) / dw - 0.5f, clamp, truncate, and the sum of
-// four products ((c * wx) * wy) added left to right.
-__device__ __forceinline__ void resize_axis(unsigned i, unsigned sdim, unsigned ddim, unsigned &i0,
-                                            unsigned &i1, float &frac) {
-  float s = __fsub_rn(__fdiv_rn(__fmul_rn(__fadd_rn((float)i, 0.5f), (float)sdim), (float)ddim), 0.5f);
-  const float hi = __fsub_rn((float)sdim, 1.0f);
-  s = s < hi ? s : hi;
-  s = 0.0f > s ? 0.0f : s;
-  i0 = __float2uint_rz(s);
-  i1 = i0 + 1 < sdim - 1 ? i0 + 1 : sdim - 1;
-  frac = __fsub_rn(s, (float)i0);
-}
-
+// (resize_axis and bilerp, in resample.cuh)
 // A thread produces 4 adjacent dst pixels for RS_ROWS rows: the x-axis coefficients (two IEEE
 // divisions per pixel in the reference's formula) are computed once per thread, the y-axis ones once
 // per row, and the 4 results leave as one 32-bit store.
@@ -61,14 +49,6 @@ __device__ __forceinline__ void resize_axis(unsigned i, unsigned sdim, unsigned 
 // of the loaded words.  Threads that do not qualify (other ratios, clamped edges) take the gather path.
 constexpr int RS_ROWS = 8;
 
-__device__ __forceinline__ float bilerp(float c00, float c01, float c10, float c11, float omx, float dx, float omy,
-                                        float dy) {
-  float p = __fmul_rn(__fmul_rn(c00, omx), omy);                  // reference :181-184, left to right
-  p = __fadd_rn(p, __fmul_rn(__fmul_rn(c01, dx), omy));
-  p = __fadd_rn(p, __fmul_rn(__fmul_rn(c10, omx), dy));
-  p = __fadd_rn(p, __fmul_rn(__fmul_rn(c11, dx), dy));
-  return p;
-}
 // u8 -> f32 and f32 -> u8 without the conversion pipe (I2F / F2I run at 16 lanes/clk/SM and four conversions per
 // dst pixel capped round 1's kernel at ~4 pixels/clk/SM): adding 2^23 to p in [0, 256) with round-toward-zero leaves
 // trunc(p) in the low byte.
