@@ -15,11 +15,20 @@
  *   blobs:N         (prints the number of 4-connected components >= 128 per frame; frames pass through unchanged)
  *   scan:W:H        (the reference's document scanner, nanomagick.c:186-210, per frame on the device: blur 1 ->
  *                    Otsu + 10 threshold -> blobs -> corners of the largest blob -> perspective warp to W x H)
+ *   orb:TEMPLATE.pgm (the reference's orb verb, nanomagick.c:292-311: pyramid ORB of the template and of every frame,
+ *                    2500 keypoints, threshold 20, 3 levels, then gs_match_orb with at most 300 matches at distance
+ *                    60; prints "frame F: Template: T keypoints, Scene: S keypoints, Matches: M" per frame and passes
+ *                    the frames through unchanged.  The verb runs both extractions in one static 1 MiB buffer, so a
+ *                    frame's score maps start with the bytes the template call left at their offsets; the stage
+ *                    reproduces that.  When the template's or a frame's pyramid and score maps need more than 1 MiB
+ *                    the verb overruns its buffer and its result is undefined; the stage then starts from zeroed maps.
+ *                    The matches are not drawn.)
  * e.g. the reference Makefile's lena chain:  blur:2,threshold:otsu,erode:2,dilate:2
  * Stage semantics are the reference's gs_* functions (same kernels as the drop-in gs_* entry points).
  */
 #include <string.h>
 
+#include "grayskull_b200_pyramid.h"
 #include "grayskull_b200_roi.h"
 
 #define DIE(...) (fprintf(stderr, "gsb_magick: " __VA_ARGS__), fprintf(stderr, "\n"), exit(1))
@@ -44,6 +53,98 @@ static void ensure(struct batch *b, unsigned w, unsigned h, unsigned n, size_t *
     *cap = need;
   }
   b->w = w, b->h = h, b->n = n;
+}
+
+/* bytes of pyramid levels 1..L-1 and of score maps 0..L-1 of one w x h image (nanomagick.c:255-270), and the offset
+ * of level l's score map among the score maps */
+static size_t pyr_bytes(unsigned w, unsigned h, unsigned L, size_t *maps, size_t off[4]) {
+  size_t pyr = 0, sm = 0;
+  unsigned l;
+  for (l = 0; l < L; l++, w /= 2, h /= 2) {
+    off[l] = sm;
+    sm += (size_t)w * h;
+    if (l) pyr += (size_t)w * h;
+  }
+  *maps = sm;
+  return pyr;
+}
+
+/* the orb stage (see the header comment): template as set 1 of every pair, frame f's keypoints as set 2 */
+static void orb_stage(const char *path, const struct batch *cur) {
+  enum { NK = 2500, TH = 20, LV = 3, MM = 300 };
+  const size_t BUF = 1024 * 1024; /* nanomagick.c:299 */
+  unsigned w = cur->w, h = cur->h, n = cur->n, f, l, tl, sl, ht, *tcount, *scount, *n1, *mcount, *hs, *hm, *h1;
+  size_t tmaps, smaps, toff[4], soff[4], tpyr, spyr;
+  struct gs_keypoint *tk, *tks, *sk, *htk;
+  struct gs_match *matches;
+  uint8_t *tdev, *tbuf, *spyrd, *ssm;
+  int stale;
+  struct gs_image tpl = gs_read_pgm(path);
+  if (!gs_valid(tpl)) DIE("could not load template %s", path);
+  tl = gs_b200_orb_pyramid_levels(tpl.w, tpl.h, LV);
+  sl = gs_b200_orb_pyramid_levels(w, h, LV);
+  tpyr = pyr_bytes(tpl.w, tpl.h, tl, &tmaps, toff);
+  spyr = pyr_bytes(w, h, sl, &smaps, soff);
+  stale = tpyr + tmaps <= BUF && spyr + smaps <= BUF;
+  tdev = (uint8_t *)gs_b200_malloc((size_t)tpl.w * tpl.h);
+  tbuf = (uint8_t *)gs_b200_malloc(tpyr + tmaps > BUF ? tpyr + tmaps : BUF);
+  tk = (struct gs_keypoint *)gs_b200_malloc(sizeof(*tk) * NK);
+  tks = (struct gs_keypoint *)gs_b200_malloc(sizeof(*tks) * NK * (size_t)n);
+  tcount = (unsigned *)gs_b200_malloc(sizeof(unsigned));
+  spyrd = spyr ? (uint8_t *)gs_b200_malloc(spyr * n) : NULL;
+  ssm = (uint8_t *)gs_b200_malloc(smaps * n);
+  sk = (struct gs_keypoint *)gs_b200_malloc(sizeof(*sk) * NK * (size_t)n);
+  scount = (unsigned *)gs_b200_malloc(sizeof(unsigned) * n);
+  n1 = (unsigned *)gs_b200_malloc(sizeof(unsigned) * n);
+  matches = (struct gs_match *)gs_b200_malloc(sizeof(*matches) * MM * (size_t)n);
+  mcount = (unsigned *)gs_b200_malloc(sizeof(unsigned) * n);
+  htk = (struct gs_keypoint *)malloc(sizeof(*htk) * NK * (size_t)n);
+  hs = (unsigned *)malloc(sizeof(unsigned) * n);
+  hm = (unsigned *)malloc(sizeof(unsigned) * n);
+  h1 = (unsigned *)malloc(sizeof(unsigned) * n);
+  if (!tdev || !tbuf || !tk || !tks || !tcount || (spyr && !spyrd) || !ssm || !sk || !scount || !n1 || !matches ||
+      !mcount || !htk || !hs || !hm || !h1)
+    DIE("allocation failed");
+  /* the template call, into the zeroed buffer laid out as nanomagick lays it out: pyramid, then score maps */
+  CK(gs_b200_memcpy_h2d(tdev, tpl.data, (size_t)tpl.w * tpl.h, NULL));
+  CK(gs_b200_memset(tbuf, 0, tpyr + tmaps > BUF ? tpyr + tmaps : BUF, NULL));
+  CK(gs_b200_orb_pyramid_batch(tdev, tpl.w, tpl.h, 1, LV, tpyr ? tbuf : NULL, tbuf + tpyr, tk, tcount, NK, TH, NULL));
+  if (stale) { /* frame f's level-l map starts as the buffer's bytes at the scene's offset of that map */
+    uint8_t *hbuf = (uint8_t *)malloc(BUF), *hmaps = (uint8_t *)malloc(smaps * n);
+    if (!hbuf || !hmaps) DIE("allocation failed");
+    CK(gs_b200_memcpy_d2h(hbuf, tbuf, BUF, NULL));
+    CK(gs_b200_stream_sync(NULL));
+    for (l = 0; l < sl; l++) {
+      size_t lb = (size_t)(w >> l) * (h >> l);
+      for (f = 0; f < n; f++) memcpy(hmaps + soff[l] * n + lb * f, hbuf + spyr + soff[l], lb);
+    }
+    CK(gs_b200_memcpy_h2d(ssm, hmaps, smaps * n, NULL));
+    CK(gs_b200_stream_sync(NULL));
+    free(hbuf), free(hmaps);
+  } else {
+    CK(gs_b200_memset(ssm, 0, smaps * n, NULL));
+  }
+  CK(gs_b200_orb_pyramid_batch(cur->dev, w, h, n, LV, spyrd, ssm, sk, scount, NK, TH, NULL));
+  /* the template's list as set 1 of each of the n pairs */
+  CK(gs_b200_memcpy_d2h(htk, tk, sizeof(*tk) * NK, NULL));
+  CK(gs_b200_memcpy_d2h(&ht, tcount, sizeof(unsigned), NULL));
+  CK(gs_b200_stream_sync(NULL));
+  for (f = 0; f < n; f++) {
+    if (f) memcpy(htk + (size_t)NK * f, htk, sizeof(*htk) * NK);
+    h1[f] = ht;
+  }
+  CK(gs_b200_memcpy_h2d(tks, htk, sizeof(*htk) * NK * (size_t)n, NULL));
+  CK(gs_b200_memcpy_h2d(n1, h1, sizeof(unsigned) * n, NULL));
+  CK(gs_b200_match_orb_batch(tks, n1, NK, sk, scount, NK, n, matches, mcount, MM, 60.0f, NULL));
+  CK(gs_b200_memcpy_d2h(hs, scount, sizeof(unsigned) * n, NULL));
+  CK(gs_b200_memcpy_d2h(hm, mcount, sizeof(unsigned) * n, NULL));
+  CK(gs_b200_stream_sync(NULL));
+  for (f = 0; f < n; f++) printf("frame %u: Template: %u keypoints, Scene: %u keypoints, Matches: %u\n", f, ht, hs[f], hm[f]);
+  gs_b200_free(tdev), gs_b200_free(tbuf), gs_b200_free(tk), gs_b200_free(tks), gs_b200_free(tcount);
+  if (spyrd) gs_b200_free(spyrd);
+  gs_b200_free(ssm), gs_b200_free(sk), gs_b200_free(scount), gs_b200_free(n1), gs_b200_free(matches);
+  gs_b200_free(mcount), free(htk), free(hs), free(hm), free(h1);
+  gs_free(tpl);
 }
 
 /* one stage: reads *cur, leaves the result in *cur (swapping with *tmp when the op is out of place) */
@@ -109,6 +210,9 @@ static void stage(const char *spec, struct batch *cur, struct batch *tmp, size_t
     roi.x = (unsigned)x, roi.y = (unsigned)y, roi.w = (unsigned)cw, roi.h = (unsigned)ch;
     ensure(tmp, roi.w, roi.h, n, cap_tmp);
     CK(gs_b200_crop_resize_batch(tmp->dev, roi.w, roi.h, cur->dev, w, h, n, roi, GS_B200_NEAREST, NULL));
+  } else if (!strncmp(spec, "orb:", 4) && spec[4]) {
+    swap = 0;
+    orb_stage(spec + 4, cur);
   } else if (!strcmp(name, "keypoints") && nargs == 2) {
     unsigned nk = (unsigned)atoi(a0), f, *counts, *hc;
     struct gs_keypoint *kps;

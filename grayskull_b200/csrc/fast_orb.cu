@@ -995,6 +995,11 @@ int gs_b200_fast_batch(const uint8_t *src, unsigned w, unsigned h, unsigned n, u
                         threshold, static_cast<cudaStream_t>(s));
 }
 
+int gsb_orb_select(const struct gs_keypoint *cand, const unsigned *cand_count, unsigned cap, unsigned w, unsigned h,
+                   struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned n, cudaStream_t st);
+int gsb_orb_describe(const uint8_t *src, unsigned w, unsigned h, struct gs_keypoint *kps, const unsigned *counts,
+                     unsigned nkps, unsigned n, cudaStream_t st);
+
 int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsigned n, uint8_t *scoremap,
                               struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned threshold,
                               gs_b200_stream s) {
@@ -1008,7 +1013,22 @@ int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsign
   if (!cand || !ccount) return gsb::workspace_error();
   int rc = gsb::fast_impl(src, w, h, n, scoremap, w, h, cand, ccount, cap, threshold, st);
   if (rc) return rc;
-  GSB_LAUNCH(gsb::k_orb_select, n, 256, 0, st, cand, ccount, cap, w, h, reinterpret_cast<gsb::KpRec *>(kps), counts, nkps);
+  if ((rc = gsb_orb_select(reinterpret_cast<const struct gs_keypoint *>(cand), ccount, cap, w, h, kps, counts, nkps, n, st))) return rc;
+  return gsb_orb_describe(src, w, h, kps, counts, nkps, n, st);
+}
+
+// gs_orb_extract's two steps after FAST, also the hooks of libgrayskull_b200_pyramid.so:
+// select: cand = n lists of stride `cap` (FAST's output) with cand_count[f] entries (at most cap are read) -> at most
+// nkps response-sorted candidates 15 px inside the frame at kps + f*nkps, their number in counts[f];
+// describe: angle and BRIEF-256 of the first counts[f] records of each list, on frame f of src.
+int gsb_orb_select(const struct gs_keypoint *cand, const unsigned *cand_count, unsigned cap, unsigned w, unsigned h,
+                   struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned n, cudaStream_t st) {
+  GSB_LAUNCH(gsb::k_orb_select, n, 256, 0, st, reinterpret_cast<const gsb::KpRec *>(cand), cand_count, cap, w, h,
+             reinterpret_cast<gsb::KpRec *>(kps), counts, nkps);
+  return 0;
+}
+int gsb_orb_describe(const uint8_t *src, unsigned w, unsigned h, struct gs_keypoint *kps, const unsigned *counts,
+                     unsigned nkps, unsigned n, cudaStream_t st) {
   const unsigned long long warps = (unsigned long long)n * nkps;
   const unsigned long long blocks = (warps + 7) / 8;
   GSB_ASSERT(blocks < 0x7FFFFFFFull);
