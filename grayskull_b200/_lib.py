@@ -1,5 +1,6 @@
-"""ctypes binding of libgrayskull_b200.so -- every symbol declared in include/grayskull.h and
-include/grayskull_b200.h.  There is no fallback: if the library is missing this raises."""
+"""ctypes binding of libgrayskull_b200.so -- every symbol declared in include/grayskull.h,
+include/grayskull_b200.h, include/grayskull_b200_roi.h and include/grayskull_b200_pyramid.h.  There is no fallback: if
+the library is missing this raises."""
 import ctypes as C
 import os
 
@@ -122,6 +123,12 @@ SIGNATURES = {
     "gs_b200_match_orb_batch": (_i, [_p, _p, _u, _p, _p, _u, _u, _p, _p, _u, _f, _p]),
     "gs_b200_lbp_detect_batch": (_i, [_p, _p, _u, _u, _u, _p, _p, _u, _f, _f, _f, _i, _p]),
     "gs_b200_lbp_window_count": (C.c_ulonglong, [_p, _u, _u, _f, _f, _f, _i]),
+    # include/grayskull_b200_roi.h
+    "gs_b200_crop_resize_batch": (_i, [_p, _u, _u, _p, _u, _u, _u, Rect, _i, _p]),
+    "gs_b200_rois_resize_batch": (_i, [_p, _u, _u, _p, _u, _u, _u, _p, _p, _u, _i, _p]),
+    # include/grayskull_b200_pyramid.h
+    "gs_b200_orb_pyramid_levels": (_u, [_u, _u, _u]),
+    "gs_b200_orb_pyramid_batch": (_i, [_p, _u, _u, _u, _u, _p, _p, _p, _p, _u, _u, _p]),
 }
 
 _lib = None

@@ -12,14 +12,15 @@
 
 #include "common.cuh"
 
-extern "C" {
-int gsb_fast_single(const uint8_t *src, unsigned w, unsigned h, uint8_t *score, unsigned sw, unsigned sh,
-                    struct gs_keypoint *kps, unsigned *count, unsigned nkps, unsigned threshold, cudaStream_t s);
-int gsb_orient_single(const uint8_t *img, unsigned w, unsigned x, unsigned y, unsigned r, float *out, cudaStream_t s);
-int gsb_brief_single(const uint8_t *img, unsigned w, unsigned h, struct gs_keypoint *kp, cudaStream_t s);
-int gsb_lbp_window_single(const struct gs_lbp_cascade *c, const uint32_t *ii, unsigned iw, unsigned ih, int x, int y,
-                          float scale, unsigned *out_dev, cudaStream_t s);
-}
+namespace gsb {
+// fast_orb.cu, lbp.cu
+int fast_single(const uint8_t *src, unsigned w, unsigned h, uint8_t *score, unsigned sw, unsigned sh,
+                struct gs_keypoint *kps, unsigned *count, unsigned nkps, unsigned threshold, cudaStream_t s);
+int orient_single(const uint8_t *img, unsigned w, unsigned x, unsigned y, unsigned r, float *out, cudaStream_t s);
+int brief_single(const uint8_t *img, unsigned w, unsigned h, struct gs_keypoint *kp, cudaStream_t s);
+int lbp_window_single(const struct gs_lbp_cascade *c, const uint32_t *ii, unsigned iw, unsigned ih, int x, int y,
+                      float scale, unsigned *out_dev, cudaStream_t s);
+}  // namespace gsb
 
 namespace {
 
@@ -183,8 +184,8 @@ unsigned gs_fast(struct gs_image img, struct gs_image scoremap, struct gs_keypoi
   unsigned *cnt = static_cast<unsigned *>(gsb::workspace(S(), gsb::WS_STAGE_D, 256));
   if (!cnt) die("device workspace allocation", 1);
   uint8_t *mp = sw ? (uint8_t *)m.dev : (uint8_t *)cnt;  // never dereferenced when sw == 0
-  GS_DO(gsb_fast_single((const uint8_t *)s.dev, img.w, img.h, mp, sw, sh, (struct gs_keypoint *)k.dev, cnt, nkps,
-                        threshold, S()));
+  GS_DO(gsb::fast_single((const uint8_t *)s.dev, img.w, img.h, mp, sw, sh, (struct gs_keypoint *)k.dev, cnt, nkps,
+                         threshold, S()));
   unsigned n = 0;
   GS_CUDA(cudaMemcpyAsync(&n, cnt, sizeof(n), cudaMemcpyDeviceToHost, S()));
   finish();
@@ -199,7 +200,7 @@ float gs_compute_orientation(struct gs_image img, unsigned x, unsigned y, unsign
   Buf s = in_buf(img.data, (size_t)img.w * img.h, gsb::WS_STAGE_A);
   float *out = static_cast<float *>(gsb::workspace(S(), gsb::WS_STAGE_D, 256));
   if (!out) die("device workspace allocation", 1);
-  GS_DO(gsb_orient_single((const uint8_t *)s.dev, img.w, x, y, r, out, S()));
+  GS_DO(gsb::orient_single((const uint8_t *)s.dev, img.w, x, y, r, out, S()));
   float a = 0;
   GS_CUDA(cudaMemcpyAsync(&a, out, sizeof(a), cudaMemcpyDeviceToHost, S()));
   finish();
@@ -210,7 +211,7 @@ void gs_brief_descriptor(struct gs_image img, struct gs_keypoint *kp) {
   GSB_ASSERT(gs_ok(img) && kp);  // reference :624
   Buf s = in_buf(img.data, (size_t)img.w * img.h, gsb::WS_STAGE_A);
   Buf k = in_buf(kp, sizeof(struct gs_keypoint), gsb::WS_STAGE_C, true);
-  GS_DO(gsb_brief_single((const uint8_t *)s.dev, img.w, img.h, (struct gs_keypoint *)k.dev, S()));
+  GS_DO(gsb::brief_single((const uint8_t *)s.dev, img.w, img.h, (struct gs_keypoint *)k.dev, S()));
   out_buf(k);
   finish();
 }
@@ -391,7 +392,7 @@ unsigned gs_lbp_window(const struct gs_lbp_cascade *c, const unsigned *ii, unsig
   Buf t = in_buf(ii, (size_t)iw * ih * 4, gsb::WS_STAGE_A);
   unsigned *out = static_cast<unsigned *>(gsb::workspace(S(), gsb::WS_STAGE_D, 256));
   if (!out) die("device workspace allocation", 1);
-  GS_DO(gsb_lbp_window_single(c, (const uint32_t *)t.dev, iw, ih, x, y, scale, out, S()));
+  GS_DO(gsb::lbp_window_single(c, (const uint32_t *)t.dev, iw, ih, x, y, scale, out, S()));
   unsigned r = 0;
   GS_CUDA(cudaMemcpyAsync(&r, out, sizeof(r), cudaMemcpyDeviceToHost, S()));
   finish();

@@ -72,8 +72,8 @@ int upload(void *dst, const void *src, size_t bytes, const char *file, int line)
 
 enum { WS_INTEGRAL = 0, WS_FAST_A, WS_FAST_B, WS_ORB_A, WS_ORB_B, WS_LBP_A, WS_LBP_B, WS_LBP_C,
        WS_STAGE_A, WS_STAGE_B, WS_STAGE_C, WS_STAGE_D, WS_HIST, WS_STAGE_FUSED, WS_BLOB_A, WS_BLOB_B, WS_BLOB_C, WS_MORPH,
-       // libgrayskull_b200_pyramid.so (through gsb_workspace): per-level keypoint lists, the last level's FAST
-       // candidates, per-level counts.  Distinct from WS_FAST_* / WS_ORB_*, which the calls it makes in between use.
+       // csrc/pyramid.cu: per-level keypoint lists, the last level's FAST candidates, per-level counts.  Distinct from
+       // WS_FAST_* / WS_ORB_*, which the calls it makes in between use.
        WS_PYR_LISTS, WS_PYR_CAND, WS_PYR_COUNTS, WS_SLOTS };
 
 // 3-D tensor map over n dense u8 frames of w x h, viewed as 32-bit words {w/4, h, n}

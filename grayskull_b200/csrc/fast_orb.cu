@@ -976,6 +976,15 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
   return 0;
 }
 
+// gs_orb_extract's two steps after FAST, also called by pyramid.cu:
+// select: cand = n lists of stride `cap` (FAST's output) with cand_count[f] entries (at most cap are read) -> at most
+// nkps response-sorted candidates 15 px inside the frame at kps + f*nkps, their number in counts[f];
+// describe: angle and BRIEF-256 of the first counts[f] records of each list, on frame f of src.
+int orb_select(const struct gs_keypoint *cand, const unsigned *cand_count, unsigned cap, unsigned w, unsigned h,
+               struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned n, cudaStream_t st);
+int orb_describe(const uint8_t *src, unsigned w, unsigned h, struct gs_keypoint *kps, const unsigned *counts,
+                 unsigned nkps, unsigned n, cudaStream_t st);
+
 }  // namespace gsb
 
 extern "C" {
@@ -995,11 +1004,6 @@ int gs_b200_fast_batch(const uint8_t *src, unsigned w, unsigned h, unsigned n, u
                         threshold, static_cast<cudaStream_t>(s));
 }
 
-int gsb_orb_select(const struct gs_keypoint *cand, const unsigned *cand_count, unsigned cap, unsigned w, unsigned h,
-                   struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned n, cudaStream_t st);
-int gsb_orb_describe(const uint8_t *src, unsigned w, unsigned h, struct gs_keypoint *kps, const unsigned *counts,
-                     unsigned nkps, unsigned n, cudaStream_t st);
-
 int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsigned n, uint8_t *scoremap,
                               struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned threshold,
                               gs_b200_stream s) {
@@ -1013,22 +1017,22 @@ int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsign
   if (!cand || !ccount) return gsb::workspace_error();
   int rc = gsb::fast_impl(src, w, h, n, scoremap, w, h, cand, ccount, cap, threshold, st);
   if (rc) return rc;
-  if ((rc = gsb_orb_select(reinterpret_cast<const struct gs_keypoint *>(cand), ccount, cap, w, h, kps, counts, nkps, n, st))) return rc;
-  return gsb_orb_describe(src, w, h, kps, counts, nkps, n, st);
+  if ((rc = gsb::orb_select(reinterpret_cast<const struct gs_keypoint *>(cand), ccount, cap, w, h, kps, counts, nkps, n, st))) return rc;
+  return gsb::orb_describe(src, w, h, kps, counts, nkps, n, st);
 }
 
-// gs_orb_extract's two steps after FAST, also the hooks of libgrayskull_b200_pyramid.so:
-// select: cand = n lists of stride `cap` (FAST's output) with cand_count[f] entries (at most cap are read) -> at most
-// nkps response-sorted candidates 15 px inside the frame at kps + f*nkps, their number in counts[f];
-// describe: angle and BRIEF-256 of the first counts[f] records of each list, on frame f of src.
-int gsb_orb_select(const struct gs_keypoint *cand, const unsigned *cand_count, unsigned cap, unsigned w, unsigned h,
-                   struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned n, cudaStream_t st) {
+}  // extern "C"
+
+namespace gsb {
+
+int orb_select(const struct gs_keypoint *cand, const unsigned *cand_count, unsigned cap, unsigned w, unsigned h,
+               struct gs_keypoint *kps, unsigned *counts, unsigned nkps, unsigned n, cudaStream_t st) {
   GSB_LAUNCH(gsb::k_orb_select, n, 256, 0, st, reinterpret_cast<const gsb::KpRec *>(cand), cand_count, cap, w, h,
              reinterpret_cast<gsb::KpRec *>(kps), counts, nkps);
   return 0;
 }
-int gsb_orb_describe(const uint8_t *src, unsigned w, unsigned h, struct gs_keypoint *kps, const unsigned *counts,
-                     unsigned nkps, unsigned n, cudaStream_t st) {
+int orb_describe(const uint8_t *src, unsigned w, unsigned h, struct gs_keypoint *kps, const unsigned *counts,
+                 unsigned nkps, unsigned n, cudaStream_t st) {
   const unsigned long long warps = (unsigned long long)n * nkps;
   const unsigned long long blocks = (warps + 7) / 8;
   GSB_ASSERT(blocks < 0x7FFFFFFFull);
@@ -1043,19 +1047,19 @@ int gsb_orb_describe(const uint8_t *src, unsigned w, unsigned h, struct gs_keypo
   return 0;
 }
 
-// internal hooks used by api.cu for the single-image calls
-int gsb_fast_single(const uint8_t *src, unsigned w, unsigned h, uint8_t *score, unsigned sw, unsigned sh,
-                    struct gs_keypoint *kps, unsigned *count, unsigned nkps, unsigned threshold, cudaStream_t s) {
+// the single-image calls of api.cu
+int fast_single(const uint8_t *src, unsigned w, unsigned h, uint8_t *score, unsigned sw, unsigned sh,
+                struct gs_keypoint *kps, unsigned *count, unsigned nkps, unsigned threshold, cudaStream_t s) {
   return gsb::fast_impl(src, w, h, 1, score, sw, sh, reinterpret_cast<gsb::KpRec *>(kps), count, nkps, threshold, s);
 }
-int gsb_orient_single(const uint8_t *img, unsigned w, unsigned x, unsigned y, unsigned r, float *out, cudaStream_t s) {
+int orient_single(const uint8_t *img, unsigned w, unsigned x, unsigned y, unsigned r, float *out, cudaStream_t s) {
   if (gsb::g_trig_mode == 0) gsb::trig_selfcheck_once(s);
   GSB_LAUNCH(gsb::k_orient_one, 1, 32, 0, s, img, w, x, y, r, gsb::g_trig_mode, out);
   return 0;
 }
-int gsb_brief_single(const uint8_t *img, unsigned w, unsigned h, struct gs_keypoint *kp, cudaStream_t s) {
+int brief_single(const uint8_t *img, unsigned w, unsigned h, struct gs_keypoint *kp, cudaStream_t s) {
   if (gsb::g_trig_mode == 0) gsb::trig_selfcheck_once(s);
   GSB_LAUNCH(gsb::k_brief_one, 1, 32, 0, s, img, w, h, reinterpret_cast<gsb::KpRec *>(kp), gsb::g_trig_mode);
   return 0;
 }
-}
+}  // namespace gsb

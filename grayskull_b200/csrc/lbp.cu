@@ -970,9 +970,13 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
   return 0;
 }
 
-// single-window hook for api.cu (gs_lbp_window): scale-specific geometry is built on the fly
-int gsb_lbp_window_single(const struct gs_lbp_cascade *c, const uint32_t *ii, unsigned iw, unsigned ih, int x, int y,
-                          float scale, unsigned *out_dev, cudaStream_t s) {
+}  // extern "C"
+
+namespace gsb {
+
+// single-window call of api.cu (gs_lbp_window): scale-specific geometry is built on the fly
+int lbp_window_single(const struct gs_lbp_cascade *c, const uint32_t *ii, unsigned iw, unsigned ih, int x, int y,
+                      float scale, unsigned *out_dev, cudaStream_t s) {
   const int nf = c->nfeatures, nw = c->nweaks, nst = c->nstages;
   const unsigned nsub = gsb::subsets_len(c);
   std::vector<short4> feat(nf);
@@ -1007,4 +1011,4 @@ int gsb_lbp_window_single(const struct gs_lbp_cascade *c, const uint32_t *ii, un
              reinterpret_cast<const gsb::Stage *>(blob + o_st), nst, out_dev);
   return 0;
 }
-}
+}  // namespace gsb

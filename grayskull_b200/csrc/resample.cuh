@@ -1,5 +1,5 @@
 // resample.cuh -- gs_resize's per-axis coordinate mapping and its four-tap sum (reference grayskull.h:174-184), shared
-// by resample.cu and the region kernels of libgrayskull_b200_roi.so (grayskull_b200/roi/roi.cu).
+// by resample.cu and the region kernels of roi.cu.
 #pragma once
 #include <cuda_runtime.h>
 

@@ -216,14 +216,6 @@ int gs_b200_uses_tma(unsigned w, unsigned h, const void *ptr) {
   return gsb::tma_ok(ptr, w) ? 1 : 0;
 }
 unsigned long long gs_b200_launch_count(void) { return gsb::g_launches.load(); }
-// Hooks of the companion libraries (libgrayskull_b200_roi.so, libgrayskull_b200_pyramid.so): each links its own cudart, so it checks its launches
-// itself and reports here, keeping one error text and one launch count for every call of the ABI.
-int gsb_record_error(int e, const char *file, int line) { return gsb::record_error(static_cast<cudaError_t>(e), file, line); }
-void gsb_count_launch(void) { gsb::g_launches.fetch_add(1, std::memory_order_relaxed); }
-// this library's workspace arenas (per stream, per thread for cudaStreamPerThread, refused growth under capture) for
-// a companion's slot of common.cuh's enum; nullptr with gsb_workspace_error() as the code when it cannot be had
-void *gsb_workspace(cudaStream_t s, int slot, size_t bytes) { return gsb::workspace(s, slot, bytes); }
-int gsb_workspace_error(void) { return gsb::workspace_error(); }
 void gs_b200_force_generic(int on) { gsb::g_force_generic = on ? 1 : 0; }
 
 void *gs_b200_malloc(size_t bytes) {

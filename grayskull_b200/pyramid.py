@@ -1,38 +1,8 @@
-"""ctypes binding of libgrayskull_b200_pyramid.so (include/grayskull_b200_pyramid.h) and its call on torch CUDA tensors:
-ORB features over an image pyramid for frame batches, bit-exact with the reference CLI's multi-scale ORB
-(extract_pyramid_orb_nm of its `orb` verb).  There is no fallback: if the library is missing this raises."""
+"""ORB features over an image pyramid for frame batches on the device (include/grayskull_b200_pyramid.h), on torch
+CUDA tensors: bit-exact with the reference CLI's multi-scale ORB (extract_pyramid_orb_nm of its `orb` verb)."""
 import ctypes as C
-import os
 
-from ._lib import HERE, check, lib as _main_lib
-
-LIB_PATH = os.path.join(HERE, "libgrayskull_b200_pyramid.so")
-
-_u, _i, _p = C.c_uint, C.c_int, C.c_void_p
-
-# name -> (restype, argtypes); the CPU test suite checks this table against include/grayskull_b200_pyramid.h
-SIGNATURES = {
-    "gs_b200_orb_pyramid_levels": (_u, [_u, _u, _u]),
-    "gs_b200_orb_pyramid_batch": (_i, [_p, _u, _u, _u, _u, _p, _p, _p, _p, _u, _u, _p]),
-}
-
-_lib = None
-
-
-def lib():
-    """Load the companion C ABI (after the main library, whose error text, launch count and workspace it uses)."""
-    global _lib
-    if _lib is None:
-        _main_lib()
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError("libgrayskull_b200_pyramid.so is not built: run `python -m grayskull_b200.build` "
-                               "(or __graft_entry__.build())")
-        handle = C.CDLL(LIB_PATH)
-        for name, (res, args) in SIGNATURES.items():
-            fn = getattr(handle, name)  # AttributeError if the symbol is missing
-            fn.restype, fn.argtypes = res, args
-        _lib = handle
-    return _lib
+from ._lib import check, lib
 
 
 def levels_for(w, h, levels):

@@ -1,39 +1,10 @@
-"""ctypes binding of libgrayskull_b200_roi.so (include/grayskull_b200_roi.h) and its calls on torch CUDA tensors:
-regions of interest cut out of frame batches and resized on the device, bit-exact with the reference's gs_crop followed
-by gs_resize_nn (NEAREST) or gs_resize (BILINEAR).  There is no fallback: if the library is missing this raises."""
+"""Regions of interest cut out of frame batches and resized on the device (include/grayskull_b200_roi.h), on torch
+CUDA tensors: bit-exact with the reference's gs_crop followed by gs_resize_nn (NEAREST) or gs_resize (BILINEAR)."""
 import ctypes as C
-import os
 
-from ._lib import HERE, Rect, check, lib as _main_lib
+from ._lib import Rect, check, lib
 
-LIB_PATH = os.path.join(HERE, "libgrayskull_b200_roi.so")
 NEAREST, BILINEAR = 0, 1   # GS_B200_NEAREST, GS_B200_BILINEAR
-
-_u, _i, _p = C.c_uint, C.c_int, C.c_void_p
-
-# name -> (restype, argtypes); the CPU test suite checks this table against include/grayskull_b200_roi.h
-SIGNATURES = {
-    "gs_b200_crop_resize_batch": (_i, [_p, _u, _u, _p, _u, _u, _u, Rect, _i, _p]),
-    "gs_b200_rois_resize_batch": (_i, [_p, _u, _u, _p, _u, _u, _u, _p, _p, _u, _i, _p]),
-}
-
-_lib = None
-
-
-def lib():
-    """Load the companion C ABI (after the main library, whose error text and launch count it reports to)."""
-    global _lib
-    if _lib is None:
-        _main_lib()
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError("libgrayskull_b200_roi.so is not built: run `python -m grayskull_b200.build` "
-                               "(or __graft_entry__.build())")
-        handle = C.CDLL(LIB_PATH)
-        for name, (res, args) in SIGNATURES.items():
-            fn = getattr(handle, name)  # AttributeError if the symbol is missing
-            fn.restype, fn.argtypes = res, args
-        _lib = handle
-    return _lib
 
 
 def _stream():

@@ -1,7 +1,6 @@
 /*
- * grayskull_b200_pyramid.h -- ORB features over an image pyramid for frame batches on the device:
- * libgrayskull_b200_pyramid.so, a companion of libgrayskull_b200.so (link both: -lgrayskull_b200_pyramid
- * -lgrayskull_b200).
+ * grayskull_b200_pyramid.h -- ORB features over an image pyramid for frame batches on the device, part of
+ * libgrayskull_b200.so (link -lgrayskull_b200).
  *
  * Each frame gets exactly what the reference CLI's multi-scale ORB (examples/nanomagick/nanomagick.c:245-290, the
  * `orb` verb's extract_pyramid_orb_nm) gives it: up to 4 levels made by gs_downsample, gs_orb_extract on each level

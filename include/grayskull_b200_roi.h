@@ -1,6 +1,6 @@
 /*
- * grayskull_b200_roi.h -- regions of interest cut out of frame batches on the device: libgrayskull_b200_roi.so,
- * a companion of libgrayskull_b200.so (link both: -lgrayskull_b200_roi -lgrayskull_b200).
+ * grayskull_b200_roi.h -- regions of interest cut out of frame batches on the device, part of libgrayskull_b200.so
+ * (link -lgrayskull_b200).
  *
  * Each output image is the reference's gs_crop (grayskull.h:154-157) of one region of a frame, followed by
  * gs_resize_nn (:164-169) or gs_resize (:171-187) of that crop to dw x dh -- bit for bit those calls made one after

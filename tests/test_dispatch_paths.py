@@ -195,6 +195,8 @@ ALLOWED = {
     r"gsb::k_lbp_window_one": "single-image gs_lbp_window; test_gpu_parity.py golden test",
     r"gsb::k_morph_(tma|rows|cols)<.*>": "erode_n / dilate_n: test_morph_iter.py runs both of its paths at pointer "
                                         "offsets and counts their launches",
+    r"gsb::k_roi_.*": "region calls: test_roi.py's DISPATCH census and its witnessed GPU cases cover every one",
+    r"gsb::k_pyr_.*": "pyramid ORB: test_orb_pyramid.py's DISPATCH census and its witnessed GPU cases cover every one",
 }
 
 

@@ -1,4 +1,4 @@
-"""CPU-only tests: the C-ABI library loads and exports every symbol include/*.h declares, the
+"""CPU-only tests: the C-ABI library loads and exports exactly the symbols include/*.h declares, the
 drop-in header compiles the reference's own callers unmodified, the exact-division constants of
 the box filter are valid for every clipped count, and the frame sharding works across ranks
 (world_size 2, gloo).  No compute call is made on the library here (there is no GPU)."""
@@ -29,12 +29,19 @@ def test_library_exports_every_declared_symbol():
     from grayskull_b200 import build, _lib
     build.build()
     handle = C.CDLL(_lib.LIB_PATH)          # loads without a GPU or a driver
-    declared = _declared("grayskull.h") + _declared("grayskull_b200.h")
+    declared = sorted(set(_declared("grayskull.h") + _declared("grayskull_b200.h") + _declared("grayskull_b200_roi.h") +
+                          _declared("grayskull_b200_pyramid.h")))
     assert len(declared) > 40
+    assert {"gs_b200_crop_resize_batch", "gs_b200_rois_resize_batch", "gs_b200_orb_pyramid_batch",
+            "gs_b200_orb_pyramid_levels"} <= set(declared)
     for name in declared:
         assert hasattr(handle, name), name
         assert name in _lib.SIGNATURES, "binding table is missing %s" % name
-    assert sorted(_lib.SIGNATURES) == sorted(set(declared))
+    assert sorted(_lib.SIGNATURES) == declared
+    # the library's ABI is exactly what the headers declare: no internal function is exported
+    nm = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    exported = sorted(line.split()[-1] for line in nm.splitlines() if " T " in line)
+    assert exported == declared, sorted(set(exported) ^ set(declared))
     lib = _lib.lib()
     assert b"sm_90a" in lib.gs_b200_version()
     assert lib.gs_b200_device_count() >= 0

@@ -1,15 +1,16 @@
-"""ORB over an image pyramid on the device (libgrayskull_b200_pyramid.so, include/grayskull_b200_pyramid.h), bit-exact
-with the reference CLI's multi-scale ORB: extract_pyramid_orb_nm of its `orb` verb.
+"""ORB over an image pyramid on the device (include/grayskull_b200_pyramid.h), bit-exact with the reference CLI's
+multi-scale ORB: extract_pyramid_orb_nm of its `orb` verb.
 
 pyramid_orb() below restates that helper from its behaviour on the oracle's gso_downsample / gso_orb_extract, with its
 one buffer (pyramid levels 1..L-1, then score maps 0..L-1) as a numpy array; orb_verb_line() restates the verb's
-printed line, the 1 MiB buffer it shares between the template and the scene included.  DISPATCH is this library's
-coverage record: every kernel of its SASS, with the cases that must launch it.
+printed line, the 1 MiB buffer it shares between the template and the scene included.  DISPATCH is the coverage record
+of the pyramid's own kernels (gsb::k_pyr_*): every one of them in the library's SASS, with the cases that must launch
+it.  test_host_logic.py checks the exports and the binding table, test_streams.py the runtime calls of pyramid.o, and
+test_dispatch_paths.py that its launches go through gsb::launch.
 
-  * CPU: the companion exports exactly what its header declares and its ctypes table binds; its SASS is sm_90a and
-    every kernel has a DISPATCH row; its object imports no blocking or legacy-stream runtime call; the level rule; the
-    restatement equals the compiled reference CLI (when oracle/_ref is built) on lena and on template / scene pairs of
-    different sizes, one of which the stale buffer changes.
+  * CPU: the pyramid kernels are sm_90a and each has a DISPATCH row; the level rule; the restatement equals the
+    compiled reference CLI (when oracle/_ref is built) on lena and on template / scene pairs of different sizes, one
+    of which the stale buffer changes.
   * GPU: every frame bit-exact against the restatement -- keypoints up to the count, untouched slots after it, every
     pyramid byte and every score-map byte with the caller's bytes as the maps' start -- at tiled and generic widths,
     L = 1..4 and a request for 5, skipped early levels, corner-rich frames whose last level's per-frame cap truncates,
@@ -19,7 +20,6 @@ coverage record: every kernel of its SASS, with the cases that must launch it.
 import ctypes as C
 import os
 import re
-import shutil
 import subprocess
 import sys
 import time
@@ -28,7 +28,7 @@ import numpy as np
 import pytest
 
 import _libs as L
-from _gpu import O, frames, kernel_id, lib, traced, witness, witnessed  # noqa: F401
+from _gpu import O, frames, lib, traced, witness, witnessed  # noqa: F401
 
 ROOT = L.ROOT
 POISON = 0xCD
@@ -119,68 +119,14 @@ def pyramid_lib():
 
 
 # ---- CPU: the library --------------------------------------------------------------------------------------------------
-def _declared(header):
-    txt = open(os.path.join(ROOT, "include", header)).read()
-    txt = txt[txt.rindex('extern "C" {'):]
-    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
-    return sorted(set(re.findall(r"\b(gs_[a-z0-9_]+)\s*\(", txt)))
-
-
-def test_companion_exports_every_declared_symbol():
-    sys.path.insert(0, ROOT)
-    from grayskull_b200 import build, pyramid
-    build.build()
-    handle = C.CDLL(pyramid.LIB_PATH)            # loads without a GPU or a driver
-    declared = _declared("grayskull_b200_pyramid.h")
-    assert declared == ["gs_b200_orb_pyramid_batch", "gs_b200_orb_pyramid_levels"]
-    for name in declared:
-        assert hasattr(handle, name), name
-    assert sorted(pyramid.SIGNATURES) == declared
-    nm = subprocess.run(["nm", "-D", "--defined-only", pyramid.LIB_PATH], capture_output=True, text=True,
-                        check=True).stdout
-    exported = sorted(line.split()[-1] for line in nm.splitlines() if " T " in line)
-    assert exported == declared, exported
-    pyramid.lib()
-
-
 def _pyr_sass():
-    from grayskull_b200 import pyramid
-    tool = L.cuda_tool("cuobjdump")
-    if tool is None:
-        pytest.skip("cuobjdump not found")
-    listing = subprocess.run([tool, "-sass", pyramid.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    funcs = {}
-    for cubin in re.split(r"^\s*(?=code for sm_\w+\s*$)", listing, flags=re.M)[1:]:
-        arch, *parts = re.split(r"^\s*Function : (\S+)\s*$", cubin, flags=re.M)
-        arch = arch.strip().splitlines()[0]
-        for name, body in zip(L.demangle(parts[0::2]), parts[1::2]):
-            funcs[kernel_id(name)] = arch + "\n" + body
-    return funcs
+    return {k: v for k, v in L.sass_functions().items() if k.startswith("gsb::k_pyr_")}
 
 
 def test_every_kernel_is_sm90a_with_a_dispatch_row():
     sass = _pyr_sass()
     assert sass and all(body.startswith("code for sm_90a\n") for body in sass.values())
     assert set(sass) == set(DISPATCH), (sorted(sass), sorted(DISPATCH))
-
-
-_BLOCKING_RE = re.compile(r"^(cudaMemcpy|cudaMemcpyToSymbol|cudaMemset|cudaMemcpy2D|cudaDeviceSynchronize|"
-                          r"cudaStreamSynchronize|cudaEventSynchronize|cudaMalloc\w*|cudaFree\w*|cudaStreamCreate\w*|"
-                          r"cudaStreamDestroy|cudaFuncSetAttribute)$")
-
-
-def test_no_blocking_runtime_calls():
-    from grayskull_b200 import build
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    objs = [os.path.join(build.OBJ, s.replace(".cu", ".o")) for s in build.PYR_SOURCES]
-    assert all(os.path.exists(o) for o in objs), objs
-    for o in objs:
-        out = subprocess.run([nm, "-u", o], capture_output=True, text=True, check=True).stdout
-        syms = [line.split()[-1] for line in out.splitlines()]
-        assert "cudaLaunchKernel" in syms and "cudaGetLastError" in syms
-        assert not [s for s in syms if _BLOCKING_RE.match(s)], syms
 
 
 def test_levels_follow_the_helper_rule():

@@ -1,14 +1,15 @@
-"""Regions of interest on the device (libgrayskull_b200_roi.so, include/grayskull_b200_roi.h): crop, then nearest or
-bilinear resize, bit-exact with the reference's gs_crop followed by gs_resize_nn or gs_resize.
+"""Regions of interest on the device (include/grayskull_b200_roi.h): crop, then nearest or bilinear resize, bit-exact
+with the reference's gs_crop followed by gs_resize_nn or gs_resize.
 
 gso_crop / gso_resize_nn below restate the reference's two calls in numpy, 32-bit wrapping arithmetic included; the
-bilinear half of the composition is the C oracle's gso_resize (tests/_libs.py).  DISPATCH is this library's coverage
-record: every kernel of its SASS, with the cases that must launch it.
+bilinear half of the composition is the C oracle's gso_resize (tests/_libs.py).  DISPATCH is the coverage record of the
+region kernels (gsb::k_roi_*): every one of them in the library's SASS, with the cases that must launch it.
+test_host_logic.py checks the exports and the binding table, test_streams.py the runtime calls of roi.o, and
+test_dispatch_paths.py that its launches go through gsb::launch.
 
-  * CPU: the companion exports exactly what its header declares and its ctypes table binds; its SASS is sm_90a and
-    every kernel has a DISPATCH row; its object imports no blocking or legacy-stream runtime call; the restatement
-    equals the reference's gs_crop / gs_resize_nn (when oracle/_ref is built), wrap cases included; the host asserts
-    abort with the reference's message and an unknown mode is an error.
+  * CPU: the region kernels are sm_90a and each has a DISPATCH row; the restatement equals the reference's gs_crop /
+    gs_resize_nn (when oracle/_ref is built), wrap cases included; the host asserts abort with the reference's message
+    and an unknown mode is an error.
   * GPU: both entry points against the composition (host regions at TMA-friendly and ragged widths, odd offsets,
     misaligned pointers; device lists with and without counts, untouched slots past the counts, invalid regions,
     a source batch over 4 GiB); LBP detection chained into the region call on the device counts; the CLI's crop
@@ -16,8 +17,6 @@ record: every kernel of its SASS, with the cases that must launch it.
 """
 import ctypes as C
 import os
-import re
-import shutil
 import subprocess
 import sys
 import time
@@ -27,7 +26,7 @@ import pytest
 
 import _libs as L
 from grayskull_b200._lib import Rect
-from _gpu import O, Region, frames, kernel_id, lib, stream, traced, witness, witnessed  # noqa: F401
+from _gpu import O, Region, frames, lib, stream, traced, witness, witnessed  # noqa: F401
 
 ROOT = L.ROOT
 NEAREST, BILINEAR = 0, 1
@@ -86,42 +85,8 @@ def roi_lib():
 
 
 # ---- CPU: the library --------------------------------------------------------------------------------------------------
-def _declared(header):
-    txt = open(os.path.join(ROOT, "include", header)).read()
-    txt = txt[txt.rindex('extern "C" {'):]
-    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
-    return sorted(set(re.findall(r"\b(gs_[a-z0-9_]+)\s*\(", txt)))
-
-
-def test_companion_exports_every_declared_symbol():
-    sys.path.insert(0, ROOT)
-    from grayskull_b200 import build, roi
-    build.build()
-    handle = C.CDLL(roi.LIB_PATH)            # loads without a GPU or a driver
-    declared = _declared("grayskull_b200_roi.h")
-    assert declared == ["gs_b200_crop_resize_batch", "gs_b200_rois_resize_batch"]
-    for name in declared:
-        assert hasattr(handle, name), name
-    assert sorted(roi.SIGNATURES) == declared
-    nm = subprocess.run(["nm", "-D", "--defined-only", roi.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    exported = sorted(line.split()[-1] for line in nm.splitlines() if " T " in line)
-    assert exported == declared, exported
-    roi.lib()
-
-
 def _roi_sass():
-    from grayskull_b200 import roi
-    tool = L.cuda_tool("cuobjdump")
-    if tool is None:
-        pytest.skip("cuobjdump not found")
-    listing = subprocess.run([tool, "-sass", roi.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    funcs = {}
-    for cubin in re.split(r"^\s*(?=code for sm_\w+\s*$)", listing, flags=re.M)[1:]:
-        arch, *parts = re.split(r"^\s*Function : (\S+)\s*$", cubin, flags=re.M)
-        arch = arch.strip().splitlines()[0]
-        for name, body in zip(L.demangle(parts[0::2]), parts[1::2]):
-            funcs[kernel_id(name)] = arch + "\n" + body
-    return funcs
+    return {k: v for k, v in L.sass_functions().items() if k.startswith("gsb::k_roi_")}
 
 
 def test_every_kernel_is_sm90a_with_a_dispatch_row():
@@ -130,25 +95,6 @@ def test_every_kernel_is_sm90a_with_a_dispatch_row():
     assert set(sass) == set(DISPATCH), (sorted(sass), sorted(DISPATCH))
     # the copy kernel moves aligned 16-byte blocks (funnel-shifted into place) and stores 16-byte chunks
     assert "LDG.E.128.CONSTANT" in sass[COPY] and "STG.E.EF.128" in sass[COPY] and "SHF.R" in sass[COPY]
-
-
-_BLOCKING_RE = re.compile(r"^(cudaMemcpy|cudaMemcpyToSymbol|cudaMemset|cudaMemcpy2D|cudaDeviceSynchronize|"
-                          r"cudaStreamSynchronize|cudaEventSynchronize|cudaMalloc\w*|cudaFree\w*|cudaStreamCreate\w*|"
-                          r"cudaStreamDestroy|cudaFuncSetAttribute)$")
-
-
-def test_no_blocking_runtime_calls():
-    from grayskull_b200 import build
-    nm = shutil.which("nm")
-    if nm is None:
-        pytest.skip("nm not found")
-    objs = [os.path.join(build.OBJ, s.replace(".cu", ".o")) for s in build.ROI_SOURCES]
-    assert all(os.path.exists(o) for o in objs), objs
-    for o in objs:
-        out = subprocess.run([nm, "-u", o], capture_output=True, text=True, check=True).stdout
-        syms = [line.split()[-1] for line in out.splitlines()]
-        assert "cudaLaunchKernel" in syms and "cudaGetLastError" in syms
-        assert not [s for s in syms if _BLOCKING_RE.match(s)], syms
 
 
 # ---- CPU: the restatement against the reference ------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""Pyramid ORB (libgrayskull_b200_pyramid.so) on one GPU: one JSON line per workload.
+"""Pyramid ORB (include/grayskull_b200_pyramid.h) on one GPU: one JSON line per workload.
 
     python tools/orb_pyramid_bench.py [--workload fhd|vga|all] [--steps 10] [--warmup 2] [--check 3] [--cpu-frames 2]
 

@@ -1,4 +1,4 @@
-"""Region-of-interest kernels (libgrayskull_b200_roi.so) on one GPU: one JSON line per workload.
+"""Region-of-interest kernels (include/grayskull_b200_roi.h) on one GPU: one JSON line per workload.
 
     python tools/roi_bench.py [--iters 20] [--warmup 3]
 
