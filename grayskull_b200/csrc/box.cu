@@ -1083,19 +1083,26 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
   if (n == 0) return 0;
   // the clamped lane compare of k_box_tma / k_box_mid (box_finish) is exact only for c > INT_MIN + 255
   const bool lane_c_ok = !ADAPTIVE || cparam > INT_MIN + 255;
+  // k_box_tma, k_box_mid and k_box_wide put the frame in grid z; k_box_generic loops over frames
+  const bool banded = r >= 1 && r <= 120 && !force_generic() && w < (1u << 30) && h < (1u << 30);
+  if (banded && n > GRID_FRAMES)
+    return for_frame_groups(n, [&](unsigned f0, unsigned c) {
+      const size_t o = (size_t)f0 * w * h;
+      return launch_box<ADAPTIVE>(dst + o, src + o, w, h, c, r, cparam, s);
+    });
   CUtensorMap tmap;
   if (lane_c_ok && r >= 1 && r <= BX_RMAX && tma_ok(src, w) && tma_ok(dst, w) &&
-      n <= 65535u && make_tmap_u8frames(&tmap, src, w, h, n, BX_PW, BX_TH + 2 * r)) {
+      make_tmap_u8frames(&tmap, src, w, h, n, BX_PW, BX_TH + 2 * r)) {
     static decltype(&k_box_tma<1, ADAPTIVE>) const box_tma_fn[BX_RMAX] = {
         k_box_tma<1, ADAPTIVE>, k_box_tma<2, ADAPTIVE>, k_box_tma<3, ADAPTIVE>, k_box_tma<4, ADAPTIVE>,
         k_box_tma<5, ADAPTIVE>, k_box_tma<6, ADAPTIVE>, k_box_tma<7, ADAPTIVE>};
     // tile t covers output columns [240 t - 8, 240 t + 232)
     const unsigned tiles_x = (w + 8 + BX_STRIDE - 1) / BX_STRIDE, tiles_y = (h + BX_TH - 1) / BX_TH;
-    GSB_ASSERT(tiles_y <= 65535u);   // grid y limit (z was checked above)
+    GSB_ASSERT(tiles_y <= 65535u);   // grid y limit (z is at most one frame group)
     GSB_LAUNCH(box_tma_fn[r - 1], dim3(tiles_x, tiles_y, n), BX_THREADS, BX_SMEM, s, tmap, dst, w, h, cparam);
     return 0;
   }
-  if (r >= 1 && r <= 120 && !force_generic() && n <= 65535u && w < (1u << 30) && h < (1u << 30)) {
+  if (banded) {
     // radius-independent path: warp-autonomous 256-column segments, u32 window sums (k_box_wide)
     const int R8 = (int)((r + 7) / 8 * 8), outw = 256 - 2 * R8;
     const int strips = (int)((w + outw - 1) / outw);
@@ -1150,8 +1157,14 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
   GSB_ASSERT(dst && src && w > 0 && h > 0);  // reference :269, :307
   cudaStream_t s = static_cast<cudaStream_t>(st);
   if (n == 0 || w < 3 || h < 3) return 0;    // gs_sobel writes nothing below 3x3 (reference :308-309)
+  // k_blur_sobel_tma puts the frame in grid z, and the fall-back's scratch batch stays at one group
+  if (n > gsb::GRID_FRAMES)
+    return gsb::for_frame_groups(n, [&](unsigned f0, unsigned c) {
+      const size_t o = (size_t)f0 * w * h;
+      return gs_b200_blur_sobel_batch(dst + o, src + o, w, h, c, radius, st);
+    });
   CUtensorMap tmap;
-  if (radius >= 1 && radius <= gsb::BX_RMAX && gsb::tma_ok(src, w) && gsb::tma_ok(dst, w) && n <= 65535u &&
+  if (radius >= 1 && radius <= gsb::BX_RMAX && gsb::tma_ok(src, w) && gsb::tma_ok(dst, w) &&
       gsb::make_tmap_u8frames(&tmap, src, w, h, n, gsb::BS_PW, gsb::BS_IN_ROWS)) {
     static decltype(&gsb::k_blur_sobel_tma<1>) const blur_sobel_fn[gsb::BX_RMAX] = {
         gsb::k_blur_sobel_tma<1>, gsb::k_blur_sobel_tma<2>, gsb::k_blur_sobel_tma<3>, gsb::k_blur_sobel_tma<4>,

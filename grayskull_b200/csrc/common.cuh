@@ -48,6 +48,21 @@ int launch(const char *file, int line, void (*k)(P...), dim3 grid, dim3 block, s
   } while (0)
 #endif  // __CUDACC__
 
+// Grid y and z stop at 65535.  A call whose kernels take the frame from blockIdx.y or .z without a loop over frames
+// runs a larger batch as consecutive groups of at most GRID_FRAMES frames: for_frame_groups calls fn(f0, count) for
+// each group in order, and fn launches that group's kernels with every per-frame base advanced by f0 frames.  The
+// groups queue on the caller's stream one after the other, so per-call workspace sized for a group is reused by the
+// next one in stream order.  Returns the first non-zero result of fn (the later groups do not run), else 0.
+constexpr unsigned GRID_FRAMES = 65535u;
+template <class F>
+int for_frame_groups(unsigned n, F &&fn) {
+  for (unsigned long long f0 = 0; f0 < n; f0 += GRID_FRAMES) {
+    const unsigned long long left = n - f0;
+    if (int rc = fn(static_cast<unsigned>(f0), static_cast<unsigned>(left < GRID_FRAMES ? left : GRID_FRAMES))) return rc;
+  }
+  return 0;
+}
+
 // the reference's gs_assert (grayskull.h:94-98): message + abort
 #define GSB_ASSERT(cond)                                \
   do {                                                  \

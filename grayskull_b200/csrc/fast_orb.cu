@@ -938,6 +938,11 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
                      unsigned sh, KpRec *kps, unsigned *counts, unsigned nkps, unsigned threshold,
                      cudaStream_t s) {
   if (n == 0) return 0;
+  if (n > GRID_FRAMES)   // k_fast_tiled2 / k_nms_mask put the frame in grid z / y
+    return for_frame_groups(n, [&](unsigned f0, unsigned c) {
+      return fast_impl(src + (size_t)f0 * w * h, w, h, c, score + (size_t)f0 * sw * sh, sw, sh, kps + (size_t)f0 * nkps,
+                       counts + f0, nkps, threshold, s);
+    });
   if (w < 7 || h < 7) {  // no interior pixel: nothing written, no keypoints
     GSB_CHECK(cudaMemsetAsync(counts, 0, sizeof(unsigned) * n, s));
     return 0;
@@ -946,7 +951,7 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
   unsigned *rowcount = static_cast<unsigned *>(workspace(s, WS_FAST_A, sizeof(unsigned) * (size_t)rows * n));
   unsigned *masks = static_cast<unsigned *>(workspace(s, WS_FAST_B, sizeof(unsigned) * (size_t)rows * n * mw));
   if (!rowcount || !masks) return gsb::workspace_error();
-  GSB_ASSERT(n <= 65535u && rows <= 0x7FFFFFFFu);
+  GSB_ASSERT(rows <= 0x7FFFFFFFu);
   // thresholds above 255 (the reference computes p + t / p - t in unsigned arithmetic, :496-498, which wraps for
   // huge t) take the literal per-pixel kernel: the tiled kernel's 16-bit lane arithmetic assumes t <= 255
   if (sw == w && sh == h && !force_generic() && threshold <= 255u) {
@@ -1010,6 +1015,11 @@ int gs_b200_orb_extract_batch(const uint8_t *src, unsigned w, unsigned h, unsign
   GSB_ASSERT(src && w > 0 && h > 0 && kps && nkps > 0 && scoremap);  // reference :653
   GSB_ASSERT(counts);
   if (n == 0) return 0;
+  if (n > gsb::GRID_FRAMES)   // FAST, select and describe per frame group, on the group's candidate workspace
+    return gsb::for_frame_groups(n, [&](unsigned f0, unsigned c) {
+      const size_t o = (size_t)f0 * w * h;
+      return gs_b200_orb_extract_batch(src + o, w, h, c, scoremap + o, kps + (size_t)f0 * nkps, counts + f0, nkps, threshold, s);
+    });
   cudaStream_t st = static_cast<cudaStream_t>(s);
   const unsigned cap = nkps * 4ull < gsb::ORB_MAXC ? nkps * 4 : gsb::ORB_MAXC;  // reference :656
   gsb::KpRec *cand = static_cast<gsb::KpRec *>(gsb::workspace(st, gsb::WS_ORB_A, sizeof(gsb::KpRec) * (size_t)cap * n));

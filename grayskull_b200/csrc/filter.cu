@@ -315,9 +315,12 @@ int gs_b200_find_best_match_batch(struct gs_point *best, const uint8_t *result, 
   GSB_ASSERT(best && result && rw > 0 && rh > 0);   // reference :727
   GSB_ASSERT((unsigned long long)rw * rh < 0xFFFFFFFFull);
   if (n == 0) return 0;
-  cudaStream_t st = static_cast<cudaStream_t>(s);
-  GSB_ASSERT(n <= 65535u);
   const size_t px = (size_t)rw * rh;
+  if (n > gsb::GRID_FRAMES)   // k_best_match_partial puts the frame in grid y
+    return gsb::for_frame_groups(n, [&](unsigned f0, unsigned c) {
+      return gs_b200_find_best_match_batch(best + f0, result + (size_t)f0 * px, rw, rh, c, s);
+    });
+  cudaStream_t st = static_cast<cudaStream_t>(s);
   unsigned long long *keys = static_cast<unsigned long long *>(gsb::workspace(st, gsb::WS_HIST, sizeof(unsigned long long) * n));
   if (!keys) return gsb::workspace_error();
   GSB_CHECK(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * n, st));

@@ -908,6 +908,11 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
   GSB_ASSERT(c && ii && iw > 0 && ih > 0 && counts && step > 0);  // step <= 0 never terminates in the reference
   GSB_ASSERT(rects || max_rects == 0);
   if (n == 0) return 0;
+  if (n > gsb::GRID_FRAMES)   // the scan, count and emit kernels put the frame in grid y
+    return gsb::for_frame_groups(n, [&](unsigned f0, unsigned m) {
+      return gs_b200_lbp_detect_batch(c, ii + (size_t)f0 * iw * ih, iw, ih, m, rects ? rects + (size_t)f0 * max_rects : rects,
+                                      counts + f0, max_rects, scale_factor, min_scale, max_scale, step, s);
+    });
   cudaStream_t st = static_cast<cudaStream_t>(s);
   // a plan miss allocates and uploads synchronously, which a graph capture cannot hold
   const bool cap = gsb::capturing(st);
@@ -919,7 +924,7 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
     return 0;
   }
   const unsigned long long nblocks = (dc.total_slots + 7) / 8;
-  GSB_ASSERT(nblocks < 0x7FFFFFFFull && n <= 65535u);
+  GSB_ASSERT(nblocks < 0x7FFFFFFFull);
   unsigned *masks = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_LBP_A, 4 * (size_t)dc.total_slots * n));
   unsigned *bcount = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_LBP_B, 4 * (size_t)nblocks * n));
   if (!masks || !bcount) return gsb::workspace_error();

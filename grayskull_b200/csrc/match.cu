@@ -165,7 +165,12 @@ extern "C" int gs_b200_match_orb_batch(const struct gs_keypoint *kps1, const uns
     GSB_CHECK(cudaMemsetAsync(counts, 0, sizeof(unsigned) * npairs, st));
     return 0;
   }
-  GSB_ASSERT(npairs <= 65535u && stride1 < 0x7FFFFFFFu && stride2 < (1u << gsb::MT_IDX_BITS));
+  GSB_ASSERT(stride1 < 0x7FFFFFFFu && stride2 < (1u << gsb::MT_IDX_BITS));
+  if (npairs > gsb::GRID_FRAMES)   // k_match_best puts the pair in grid y
+    return gsb::for_frame_groups(npairs, [&](unsigned p0, unsigned m) {
+      return gs_b200_match_orb_batch(kps1 + (size_t)p0 * stride1, n1 + p0, stride1, kps2 + (size_t)p0 * stride2, n2 + p0,
+                                     stride2, m, matches + (size_t)p0 * max_matches, counts + p0, max_matches, max_distance, s);
+    });
   uint2 *cand = static_cast<uint2 *>(gsb::workspace(st, gsb::WS_ORB_A, sizeof(uint2) * (size_t)stride1 * npairs));
   if (!cand) return gsb::workspace_error();
   GSB_LAUNCH(gsb::k_match_best, dim3((stride1 + gsb::MT_QPC - 1) / gsb::MT_QPC, npairs), 256, 0, st,

@@ -113,7 +113,6 @@ int gs_b200_orb_pyramid_batch(const uint8_t *src, unsigned w, unsigned h, unsign
     return 0;
   }
   GSB_ASSERT(src && w > 0 && h > 0 && kps && scoremap);   // gs_orb_extract's assert (reference :653)
-  GSB_ASSERT(n <= 65535u);
   const unsigned L = gsb::pyr_levels(w, h, levels);
   if (L > 1) GSB_ASSERT(pyr);
   unsigned lw[gsb::PYR_MAX_LEVELS], lh[gsb::PYR_MAX_LEVELS];
@@ -128,38 +127,49 @@ int gs_b200_orb_pyramid_batch(const uint8_t *src, unsigned w, unsigned h, unsign
   }
   const unsigned q0 = nkps / L, early = q0 ? L - 1 : 0;   // levels before the last run only with a quota
   const unsigned cap = nkps * 4ull < gsb::PYR_MAXC ? nkps * 4 : gsb::PYR_MAXC;
-  const size_t early_recs = (size_t)n * q0 * (L - 1), last_recs = (size_t)n * nkps;
-  struct gs_keypoint *lists = static_cast<struct gs_keypoint *>(
-      gsb::workspace(st, gsb::WS_PYR_LISTS, sizeof(struct gs_keypoint) * (early_recs + last_recs)));
-  struct gs_keypoint *cand =
-      static_cast<struct gs_keypoint *>(gsb::workspace(st, gsb::WS_PYR_CAND, sizeof(struct gs_keypoint) * (size_t)n * cap));
-  unsigned *lcounts = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_PYR_COUNTS, sizeof(unsigned) * (size_t)n * (L + 1)));
-  if (!lists || !cand || !lcounts) return gsb::workspace_error();
-  unsigned *ccount = lcounts + (size_t)n * L;
+  // k_pyr_merge puts the frame in grid y: the call runs per frame group, each group on its frames of every level
+  // (level l of frame f is at img[l] + f * lw[l] * lh[l]) with its own workspace lists
+  return gsb::for_frame_groups(n, [&](unsigned f0, unsigned m) {
+    const uint8_t *gimg[gsb::PYR_MAX_LEVELS];
+    uint8_t *gscore[gsb::PYR_MAX_LEVELS];
+    for (unsigned l = 0; l < L; l++) {
+      const size_t o = (size_t)f0 * lw[l] * lh[l];
+      gimg[l] = img[l] + o, gscore[l] = score[l] + o;
+    }
+    const size_t early_recs = (size_t)m * q0 * (L - 1), last_recs = (size_t)m * nkps;
+    struct gs_keypoint *lists = static_cast<struct gs_keypoint *>(
+        gsb::workspace(st, gsb::WS_PYR_LISTS, sizeof(struct gs_keypoint) * (early_recs + last_recs)));
+    struct gs_keypoint *cand =
+        static_cast<struct gs_keypoint *>(gsb::workspace(st, gsb::WS_PYR_CAND, sizeof(struct gs_keypoint) * (size_t)m * cap));
+    unsigned *lcounts = static_cast<unsigned *>(gsb::workspace(st, gsb::WS_PYR_COUNTS, sizeof(unsigned) * (size_t)m * (L + 1)));
+    if (!lists || !cand || !lcounts) return gsb::workspace_error();
+    unsigned *ccount = lcounts + (size_t)m * L;
 
-  for (unsigned l = 1; l < L; l++)
-    PYR_DO(gs_b200_downsample_batch(const_cast<uint8_t *>(img[l]), img[l - 1], lw[l - 1], lh[l - 1], n, s));
+    for (unsigned l = 1; l < L; l++)
+      PYR_DO(gs_b200_downsample_batch(const_cast<uint8_t *>(gimg[l]), gimg[l - 1], lw[l - 1], lh[l - 1], m, s));
 
-  gsb::PyrLists p = {};
-  for (unsigned l = 0; l < early; l++) {
-    struct gs_keypoint *list = lists + (size_t)n * q0 * l;
-    PYR_DO(gs_b200_orb_extract_batch(img[l], lw[l], lh[l], n, score[l], list, lcounts + (size_t)n * l, q0, threshold, s));
-    p.list[l] = reinterpret_cast<const uint4 *>(list), p.count[l] = lcounts + (size_t)n * l, p.stride[l] = q0;
-  }
+    gsb::PyrLists p = {};
+    for (unsigned l = 0; l < early; l++) {
+      struct gs_keypoint *list = lists + (size_t)m * q0 * l;
+      PYR_DO(gs_b200_orb_extract_batch(gimg[l], lw[l], lh[l], m, gscore[l], list, lcounts + (size_t)m * l, q0, threshold, s));
+      p.list[l] = reinterpret_cast<const uint4 *>(list), p.count[l] = lcounts + (size_t)m * l, p.stride[l] = q0;
+    }
 
-  const unsigned t = L - 1;
-  struct gs_keypoint *last = lists + early_recs;
-  unsigned *lcount = lcounts + (size_t)n * t;
-  const dim3 fgrid((n + 255) / 256);
-  PYR_DO(gs_b200_fast_batch(img[t], lw[t], lh[t], n, score[t], cand, ccount, cap, threshold, s));
-  GSB_LAUNCH(gsb::k_pyr_quota, fgrid, 256, 0, st, ccount, lcounts, early, n, nkps, 4u, gsb::PYR_MAXC);
-  PYR_DO(gsb::orb_select(cand, ccount, cap, lw[t], lh[t], last, lcount, nkps, n, st));
-  GSB_LAUNCH(gsb::k_pyr_quota, fgrid, 256, 0, st, lcount, lcounts, early, n, nkps, 1u, 0xFFFFFFFFu);
-  PYR_DO(gsb::orb_describe(img[t], lw[t], lh[t], last, lcount, nkps, n, st));
-  p.list[t] = reinterpret_cast<const uint4 *>(last), p.count[t] = lcount, p.stride[t] = nkps;
+    const unsigned t = L - 1;
+    struct gs_keypoint *last = lists + early_recs;
+    unsigned *lcount = lcounts + (size_t)m * t;
+    const dim3 fgrid((m + 255) / 256);
+    PYR_DO(gs_b200_fast_batch(gimg[t], lw[t], lh[t], m, gscore[t], cand, ccount, cap, threshold, s));
+    GSB_LAUNCH(gsb::k_pyr_quota, fgrid, 256, 0, st, ccount, lcounts, early, m, nkps, 4u, gsb::PYR_MAXC);
+    PYR_DO(gsb::orb_select(cand, ccount, cap, lw[t], lh[t], last, lcount, nkps, m, st));
+    GSB_LAUNCH(gsb::k_pyr_quota, fgrid, 256, 0, st, lcount, lcounts, early, m, nkps, 1u, 0xFFFFFFFFu);
+    PYR_DO(gsb::orb_describe(gimg[t], lw[t], lh[t], last, lcount, nkps, m, st));
+    p.list[t] = reinterpret_cast<const uint4 *>(last), p.count[t] = lcount, p.stride[t] = nkps;
 
-  GSB_LAUNCH(gsb::k_pyr_merge, dim3((nkps + 255) / 256, n), 256, 0, st, p, L, reinterpret_cast<uint4 *>(kps), counts, nkps);
-  return 0;
+    GSB_LAUNCH(gsb::k_pyr_merge, dim3((nkps + 255) / 256, m), 256, 0, st, p, L,
+               reinterpret_cast<uint4 *>(kps) + (size_t)f0 * nkps * 3, counts + f0, nkps);
+    return 0;
+  });
 }
 
 }  // extern "C"

@@ -251,7 +251,7 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
   if (sw == 2 * dw && sh == 2 * dh && (unsigned long long)(2 * dw) * dw < (1ull << 24) &&
       (unsigned long long)(2 * dh) * dh < (1ull << 24) && !gsb::force_generic())
     return gs_b200_downsample_batch(dst, src, sw, sh, n, s);
-  dim3 grid((dw + 127) / 128, (dh + 8 * gsb::RS_ROWS - 1) / (8 * gsb::RS_ROWS), n < 65535u ? n : 65535u);
+  dim3 grid((dw + 127) / 128, (dh + 8 * gsb::RS_ROWS - 1) / (8 * gsb::RS_ROWS), n < gsb::GRID_FRAMES ? n : gsb::GRID_FRAMES);
   GSB_ASSERT(grid.y <= 65535u);
   const bool aligned8 = sw % 8 == 0 && reinterpret_cast<uintptr_t>(src) % 8 == 0;   // every source row 8-byte aligned
   const bool vec_dst = dw % 4 == 0 && reinterpret_cast<uintptr_t>(dst) % 4 == 0;
@@ -263,12 +263,21 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
     const unsigned pitch = (cols + 15) / 16 * 16;
     const size_t bytes = (size_t)pitch * rows;
     const bool pairs_case = aligned8 && sw == 2 * dw;     // exact 2:1 in x: the 64-bit pair loads of k_resize are already good
+    // one tensor map per frame group (grid z).  The first group's is made up front: a map the driver refuses takes
+    // k_resize below, before anything is queued.  The later groups differ only in base (16-byte aligned, as the first)
+    // and in a frame count no larger.
     CUtensorMap tm;
-    if (bytes <= (size_t)gsb::RT_MAX_BYTES && pitch <= 1024 && rows <= 256 && !pairs_case &&
-        gsb::tma_ok(src, sw) && n <= 65535u && gsb::make_tmap_u8frames(&tm, src, sw, sh, n, pitch / 4, rows)) {
-      GSB_LAUNCH(vec_dst ? gsb::k_resize_tiled<true> : gsb::k_resize_tiled<false>, grid, 256, bytes, static_cast<cudaStream_t>(s),
-                 tm, dst, dw, dh, sw, sh, n, pitch, rows);
-      return 0;
+    const auto group_map = [&](unsigned f0, unsigned c) {
+      return gsb::make_tmap_u8frames(&tm, src + (size_t)f0 * sw * sh, sw, sh, c, pitch / 4, rows);
+    };
+    if (bytes <= (size_t)gsb::RT_MAX_BYTES && pitch <= 1024 && rows <= 256 && !pairs_case && gsb::tma_ok(src, sw) &&
+        group_map(0, n < gsb::GRID_FRAMES ? n : gsb::GRID_FRAMES)) {
+      return gsb::for_frame_groups(n, [&](unsigned f0, unsigned c) {
+        if (f0 && !group_map(f0, c)) return gsb::record_error(cudaErrorInvalidValue, __FILE__, __LINE__);
+        grid.z = c;
+        return gsb::launch(__FILE__, __LINE__, vec_dst ? gsb::k_resize_tiled<true> : gsb::k_resize_tiled<false>, grid, 256, bytes,
+                           static_cast<cudaStream_t>(s), tm, dst + (size_t)f0 * dw * dh, dw, dh, sw, sh, c, pitch, rows);
+      });
     }
   }
   GSB_LAUNCH(vec_dst ? gsb::k_resize<true> : gsb::k_resize<false>, grid, 256, 0, static_cast<cudaStream_t>(s), dst, dw, dh, src,

@@ -8,6 +8,8 @@
  * grayskull.h:144,147), all pointers DEVICE pointers, work enqueued on `stream`
  * (a cudaStream_t passed as void*; NULL = legacy default stream) and NOT synchronised.
  * The single-image gs_* functions are the n == 1 case plus staging and a stream sync.
+ * The frame count n (npairs for gs_b200_match_orb_batch) is bounded only by device memory: batches above the
+ * grid's 65535 limit run as consecutive frame groups on the same stream, on the same kernels as smaller ones.
  *
  * Plain C99: only pointers, sizes and PODs cross this boundary.  Every function returns 0 on
  * success or a non-zero cudaError_t value (gs_b200_last_error() gives the text).  Argument
@@ -125,13 +127,14 @@ int gs_b200_filter_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned 
  * result holds n maps of (w-tw+1) x (h-th+1) bytes */
 int gs_b200_match_template_batch(uint8_t *result, const uint8_t *img, unsigned w, unsigned h, unsigned n,
                                  const uint8_t *tmpl, unsigned tw, unsigned th, gs_b200_stream s);
-/* gs_find_best_match, reference grayskull.h:725-738, per result map */
+/* gs_find_best_match, reference grayskull.h:725-738, per result map; rw * rh < 2^32 - 1 */
 int gs_b200_find_best_match_batch(struct gs_point *best, const uint8_t *result, unsigned rw, unsigned rh,
                                   unsigned n, gs_b200_stream s);
 
 /* ---- connected components / perspective warp (SURVEY.md 8f N4) ---------------------------------- */
 /* gs_blobs, reference grayskull.h:333-405, over n frames.  labels: n*w*h gs_label; blobs: n x nblobs records, frame
- * f's first counts[f] entries valid (label order), the rest untouched; counts: n unsigned.  nblobs <= 65534. */
+ * f's first counts[f] entries valid (label order), the rest untouched; counts: n unsigned.  nblobs <= 65534,
+ * w * h < 2^32 - 1. */
 int gs_b200_blobs_batch(const uint8_t *img, unsigned w, unsigned h, unsigned n, gs_label *labels,
                         struct gs_blob *blobs, unsigned *counts, unsigned nblobs, gs_b200_stream s);
 /* gs_blob_corners, reference grayskull.h:407-421: `blob` and `corners` (4 points: tl, tr, br, bl) in DEVICE memory */

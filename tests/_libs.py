@@ -449,3 +449,126 @@ def sass_functions():
                 funcs[kernel_id(name)] = arch + "\n" + body
         _cache["sass"] = funcs
     return _cache["sass"]
+
+
+# ---- the reference's gs_crop and gs_resize_nn, restated (tests/test_roi.py) ----------------------------------------------
+M32 = 0xFFFFFFFF
+
+
+def gso_crop(a, roi):
+    """gs_crop (reference grayskull.h:154-157) of frame a (h, w) to roi = (x, y, w, h): roi.x + x in 32 bits, gs_get's
+    0 outside the frame.  The caller has checked the assert."""
+    h, w = a.shape
+    x, y, rw, rh = (int(v) for v in roi)
+    cx = (x + np.arange(rw, dtype=np.int64)) & M32
+    cy = (y + np.arange(rh, dtype=np.int64)) & M32
+    out = np.zeros((rh, rw), np.uint8)
+    vx, vy = cx < w, cy < h
+    out[np.ix_(vy, vx)] = a[np.ix_(cy[vy], cx[vx])]
+    return out
+
+
+def gso_resize_nn(c, dw, dh):
+    """gs_resize_nn (reference grayskull.h:164-169): x * src.w / dst.w in 32 bits"""
+    h, w = c.shape
+    sx = ((np.arange(dw, dtype=np.int64) * w) & M32) // max(dw, 1)
+    sy = ((np.arange(dh, dtype=np.int64) * h) & M32) // max(dh, 1)
+    out = np.zeros((dh, dw), np.uint8)
+    vx, vy = sx < w, sy < h
+    out[np.ix_(vy, vx)] = c[np.ix_(sy[vy], sx[vx])]
+    return out
+
+
+def roi_valid(roi, sw, sh):
+    x, y, w, h = (int(v) for v in roi)
+    return w > 0 and h > 0 and (x + w) & M32 <= sw and (y + h) & M32 <= sh
+
+
+def composition(Od, a, roi, dw, dh, mode):
+    """gs_crop then gs_resize_nn (mode 0, GS_B200_NEAREST) / gs_resize (mode 1), one frame; an invalid region gives
+    zeros (the device lists' rule)"""
+    if not roi_valid(roi, a.shape[1], a.shape[0]):
+        return np.zeros((dh, dw), np.uint8)
+    c = gso_crop(a, roi)
+    return gso_resize_nn(c, dw, dh) if mode == 0 else o_resize(Od, np.ascontiguousarray(c), dw, dh)
+
+
+# ---- the reference CLI's pyramid ORB, restated (tests/test_orb_pyramid.py) ---------------------------------------------
+def level_rule(w, h, levels):
+    """nanomagick.c:247,255-260: min(levels, 4) levels, stopping before one with w/2 < 32 or h/2 < 32"""
+    want = min(levels, 4)
+    for lv in range(1, want):
+        w, h = w // 2, h // 2
+        if w < 32 or h < 32:
+            return lv
+    return want
+
+
+def layout(w, h, levels):
+    """([(w_l, h_l)], offsets of pyramid levels 1..L-1, offsets of score maps 0..L-1, total bytes) of the helper's
+    buffer (nanomagick.c:261-270)"""
+    sizes = [(w >> lv, h >> lv) for lv in range(level_rule(w, h, levels))]
+    off, pyr, maps = 0, [None], []
+    for lw, lh in sizes[1:]:
+        pyr.append(off)
+        off += lw * lh
+    for lw, lh in sizes:
+        maps.append(off)
+        off += lw * lh
+    return sizes, pyr, maps, off
+
+
+def pyramid_orb(Od, a, nkps, t, buf, levels, last_cap_5000=False):
+    """extract_pyramid_orb_nm(a, kps, nkps, t, buf, levels): fills buf as the helper does and returns the keypoints.
+    last_cap_5000 runs the last level with FAST's cap at 5000 whatever its quota (for the sensitivity check)."""
+    h, w = a.shape
+    sizes, pyr, maps, total = layout(w, h, levels)
+    assert total <= buf.size, "the helper would overrun its buffer"
+    nl = len(sizes)
+    imgs = [a]
+    for lv in range(1, nl):
+        lw, lh = sizes[lv]
+        v = buf[pyr[lv]:pyr[lv] + lw * lh]
+        Od.gso_downsample(ptr(v), ptr(imgs[-1]), sizes[lv - 1][0], sizes[lv - 1][1])
+        imgs.append(v.reshape(lh, lw))
+    out = []
+    for lv in range(nl):
+        q = nkps // nl if lv < nl - 1 else nkps - sum(len(k) for k in out)
+        if q == 0:
+            out.append(np.zeros(0, KP_DTYPE))
+            continue
+        lw, lh = sizes[lv]
+        sm = buf[maps[lv]:maps[lv] + lw * lh].reshape(lh, lw)
+        if last_cap_5000 and lv == nl - 1:
+            k = o_orb(Od, imgs[lv], sm, max(q, 1250), t)[:q]   # FAST cap min(4 * 1250, 5000) = 5000
+        else:
+            k = o_orb(Od, imgs[lv], sm, q, t)
+        k = k.copy()
+        k["x"] *= np.uint32(1 << lv)
+        k["y"] *= np.uint32(1 << lv)
+        out.append(k)
+    return np.concatenate(out) if out else np.zeros(0, KP_DTYPE)
+
+
+def pyramid_expected(Od, src_np, nkps, t, levels, maps_np, last_cap_5000=False):
+    """per frame: the helper on a buffer holding zeros for the pyramid and the frame's starting maps -> (kps list,
+    pyr bytes level-major, maps bytes level-major) in the device's batch layout"""
+    n, h, w = src_np.shape
+    sizes, pyr_off, map_off, total = layout(w, h, levels)
+    kl, pyr_b, map_b = [], [[] for _ in sizes], [[] for _ in sizes]
+    base = 0
+    starts = []
+    for lw, lh in sizes:
+        starts.append(base)
+        base += lw * lh * n
+    for f in range(n):
+        buf = np.zeros(total, np.uint8)
+        for lv, (lw, lh) in enumerate(sizes):
+            buf[map_off[lv]:map_off[lv] + lw * lh] = maps_np[starts[lv] + f * lw * lh:starts[lv] + (f + 1) * lw * lh]
+        kl.append(pyramid_orb(Od, src_np[f], nkps, t, buf, levels, last_cap_5000))
+        for lv, (lw, lh) in enumerate(sizes):
+            map_b[lv].append(buf[map_off[lv]:map_off[lv] + lw * lh])
+            if lv:
+                pyr_b[lv].append(buf[pyr_off[lv]:pyr_off[lv] + lw * lh])
+    pyr = np.concatenate([np.concatenate(p) for p in pyr_b[1:]]) if len(sizes) > 1 else np.zeros(0, np.uint8)
+    return kl, pyr, np.concatenate([np.concatenate(m) for m in map_b])

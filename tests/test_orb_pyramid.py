@@ -1,7 +1,7 @@
 """ORB over an image pyramid on the device (include/grayskull_b200_pyramid.h), bit-exact with the reference CLI's
 multi-scale ORB: extract_pyramid_orb_nm of its `orb` verb.
 
-pyramid_orb() below restates that helper from its behaviour on the oracle's gso_downsample / gso_orb_extract, with its
+pyramid_orb() (tests/_libs.py) restates that helper from its behaviour on the oracle's gso_downsample / gso_orb_extract, with its
 one buffer (pyramid levels 1..L-1, then score maps 0..L-1) as a numpy array; orb_verb_line() restates the verb's
 printed line, the 1 MiB buffer it shares between the template and the scene included.  DISPATCH is the coverage record
 of the pyramid's own kernels (gsb::k_pyr_*): every one of them in the library's SASS, with the cases that must launch
@@ -28,6 +28,7 @@ import numpy as np
 import pytest
 
 import _libs as L
+from _libs import layout, level_rule, pyramid_orb
 from _gpu import O, frames, lib, traced, witness, witnessed  # noqa: F401
 
 ROOT = L.ROOT
@@ -44,63 +45,7 @@ DISPATCH = {
 BUF = 1024 * 1024        # nanomagick.c:299
 
 
-# ---- the reference CLI's pyramid ORB, restated ------------------------------------------------------------------------
-def level_rule(w, h, levels):
-    """nanomagick.c:247,255-260: min(levels, 4) levels, stopping before one with w/2 < 32 or h/2 < 32"""
-    want = min(levels, 4)
-    for lv in range(1, want):
-        w, h = w // 2, h // 2
-        if w < 32 or h < 32:
-            return lv
-    return want
-
-
-def layout(w, h, levels):
-    """([(w_l, h_l)], offsets of pyramid levels 1..L-1, offsets of score maps 0..L-1, total bytes) of the helper's
-    buffer (nanomagick.c:261-270)"""
-    sizes = [(w >> lv, h >> lv) for lv in range(level_rule(w, h, levels))]
-    off, pyr, maps = 0, [None], []
-    for lw, lh in sizes[1:]:
-        pyr.append(off)
-        off += lw * lh
-    for lw, lh in sizes:
-        maps.append(off)
-        off += lw * lh
-    return sizes, pyr, maps, off
-
-
-def pyramid_orb(Od, a, nkps, t, buf, levels, last_cap_5000=False):
-    """extract_pyramid_orb_nm(a, kps, nkps, t, buf, levels): fills buf as the helper does and returns the keypoints.
-    last_cap_5000 runs the last level with FAST's cap at 5000 whatever its quota (for the sensitivity check)."""
-    h, w = a.shape
-    sizes, pyr, maps, total = layout(w, h, levels)
-    assert total <= buf.size, "the helper would overrun its buffer"
-    nl = len(sizes)
-    imgs = [a]
-    for lv in range(1, nl):
-        lw, lh = sizes[lv]
-        v = buf[pyr[lv]:pyr[lv] + lw * lh]
-        Od.gso_downsample(L.ptr(v), L.ptr(imgs[-1]), sizes[lv - 1][0], sizes[lv - 1][1])
-        imgs.append(v.reshape(lh, lw))
-    out = []
-    for lv in range(nl):
-        q = nkps // nl if lv < nl - 1 else nkps - sum(len(k) for k in out)
-        if q == 0:
-            out.append(np.zeros(0, L.KP_DTYPE))
-            continue
-        lw, lh = sizes[lv]
-        sm = buf[maps[lv]:maps[lv] + lw * lh].reshape(lh, lw)
-        if last_cap_5000 and lv == nl - 1:
-            k = L.o_orb(Od, imgs[lv], sm, max(q, 1250), t)[:q]   # FAST cap min(4 * 1250, 5000) = 5000
-        else:
-            k = L.o_orb(Od, imgs[lv], sm, q, t)
-        k = k.copy()
-        k["x"] *= np.uint32(1 << lv)
-        k["y"] *= np.uint32(1 << lv)
-        out.append(k)
-    return np.concatenate(out) if out else np.zeros(0, L.KP_DTYPE)
-
-
+# ---- the reference CLI's orb verb, restated ------------------------------------------------------------------------------
 def orb_verb_line(Od, tpl, scene, stale=True):
     """the line the orb verb prints (nanomagick.c:299-311).  stale: one zeroed 1 MiB buffer shared by both calls, as
     there; otherwise each call gets a zeroed buffer of its own."""
@@ -273,30 +218,6 @@ def _run(lp, src_np, nkps, t, levels, maps_np):
     return rc, counts.cpu().numpy(), kps.cpu().numpy(), pyr.cpu().numpy()[:below], sm.cpu().numpy()[:maps_np.size], seen
 
 
-def expected(Od, src_np, nkps, t, levels, maps_np, last_cap_5000=False):
-    """per frame: the helper on a buffer holding zeros for the pyramid and the frame's starting maps -> (kps list,
-    pyr bytes level-major, maps bytes level-major) in the device's batch layout"""
-    n, h, w = src_np.shape
-    sizes, pyr_off, map_off, total = layout(w, h, levels)
-    kl, pyr_b, map_b = [], [[] for _ in sizes], [[] for _ in sizes]
-    base = 0
-    starts = []
-    for lw, lh in sizes:
-        starts.append(base)
-        base += lw * lh * n
-    for f in range(n):
-        buf = np.zeros(total, np.uint8)
-        for lv, (lw, lh) in enumerate(sizes):
-            buf[map_off[lv]:map_off[lv] + lw * lh] = maps_np[starts[lv] + f * lw * lh:starts[lv] + (f + 1) * lw * lh]
-        kl.append(pyramid_orb(Od, src_np[f], nkps, t, buf, levels, last_cap_5000))
-        for lv, (lw, lh) in enumerate(sizes):
-            map_b[lv].append(buf[map_off[lv]:map_off[lv] + lw * lh])
-            if lv:
-                pyr_b[lv].append(buf[pyr_off[lv]:pyr_off[lv] + lw * lh])
-    pyr = np.concatenate([np.concatenate(p) for p in pyr_b[1:]]) if len(sizes) > 1 else np.zeros(0, np.uint8)
-    return kl, pyr, np.concatenate([np.concatenate(m) for m in map_b])
-
-
 def _check(c, counts, kps, pyr, maps, want):
     kl, wpyr, wmaps = want
     nkps = c["nkps"]
@@ -326,7 +247,7 @@ def test_pyramid_vs_restatement(lib, O, witness, c):
     nmaps = sum(a * b for a, b in sizes) * n
     maps = (np.random.default_rng(w + h).integers(0, 256, nmaps, dtype=np.uint8) if c["maps"] == "random"
             else np.zeros(nmaps, np.uint8))
-    want = expected(O, src, c["nkps"], c["t"], c["levels"], maps)
+    want = L.pyramid_expected(O, src, c["nkps"], c["t"], c["levels"], maps)
 
     def run():
         lib.gs_b200_set_trig_mode(c["trig"])
@@ -341,7 +262,7 @@ def test_pyramid_vs_restatement(lib, O, witness, c):
     witnessed(witness, run, kernels, "orb_pyramid %s" % c)
     if c["kind"] == "rich":
         # the last level's per-frame cap truncates: with cap 5000 its list would differ
-        capped = expected(O, src, c["nkps"], c["t"], c["levels"], maps, last_cap_5000=True)[0]
+        capped = L.pyramid_expected(O, src, c["nkps"], c["t"], c["levels"], maps, last_cap_5000=True)[0]
         for f in range(n):
             assert capped[f].tobytes() != want[0][f].tobytes(), "frame %d: the last level's cap did not truncate" % f
 
@@ -375,7 +296,7 @@ def test_python_wrapper(lib, O):
     kps, counts, sm, pyr = pyramid.orb_pyramid_batch(torch.from_numpy(a).cuda(), 500, 20, levels=3)
     torch.cuda.synchronize()
     got = api.kps_to_numpy(kps, counts)
-    kl, wpyr, wmaps = expected(O, a, 500, 20, 3, np.zeros(sm.numel(), np.uint8))
+    kl, wpyr, wmaps = L.pyramid_expected(O, a, 500, 20, 3, np.zeros(sm.numel(), np.uint8))
     for f in range(2):
         assert got[f].tobytes() == kl[f].tobytes(), f
     assert np.array_equal(pyr.cpu().numpy(), wpyr) and np.array_equal(sm.cpu().numpy(), wmaps)
@@ -452,7 +373,7 @@ class StreamRun:
     def verify(self, got, seed):
         counts, kps, pyr, sm = (t.cpu().numpy() for t in got)
         c = dict(nkps=self.nkps, trig=0)
-        want = expected(L.oracle(), self.data[seed], self.nkps, 20, self.levels, self.maps0[seed])
+        want = L.pyramid_expected(L.oracle(), self.data[seed], self.nkps, 20, self.levels, self.maps0[seed])
         _check(c, counts, kps, pyr[:self.below], sm, want)
 
 

@@ -1,7 +1,7 @@
 """Regions of interest on the device (include/grayskull_b200_roi.h): crop, then nearest or bilinear resize, bit-exact
 with the reference's gs_crop followed by gs_resize_nn or gs_resize.
 
-gso_crop / gso_resize_nn below restate the reference's two calls in numpy, 32-bit wrapping arithmetic included; the
+gso_crop / gso_resize_nn (tests/_libs.py) restate the reference's two calls in numpy, 32-bit wrapping arithmetic included; the
 bilinear half of the composition is the C oracle's gso_resize (tests/_libs.py).  DISPATCH is the coverage record of the
 region kernels (gsb::k_roi_*): every one of them in the library's SASS, with the cases that must launch it.
 test_host_logic.py checks the exports and the binding table, test_streams.py the runtime calls of roi.o, and
@@ -25,12 +25,12 @@ import numpy as np
 import pytest
 
 import _libs as L
+from _libs import M32, composition, gso_crop, gso_resize_nn, roi_valid  # noqa: F401
 from grayskull_b200._lib import Rect
 from _gpu import O, Region, frames, lib, stream, traced, witness, witnessed  # noqa: F401
 
 ROOT = L.ROOT
 NEAREST, BILINEAR = 0, 1
-M32 = 0xFFFFFFFF
 FILL = 0xA5
 COPY, NN, BL = "gsb::k_roi_copy", "gsb::k_roi_gather<0>", "gsb::k_roi_gather<1>"
 # kernel -> the cases of this file that must launch it (test ids), checked by the census below
@@ -39,44 +39,6 @@ DISPATCH = {
     NN: ("test_crop_resize_vs_oracle[nn-*]", "test_rois_resize_vs_oracle[nearest-*]"),
     BL: ("test_crop_resize_vs_oracle[bl-*]", "test_rois_resize_vs_oracle[bilinear-*]"),
 }
-
-
-# ---- the reference's gs_crop and gs_resize_nn, restated ----------------------------------------------------------------
-def gso_crop(a, roi):
-    """gs_crop (reference grayskull.h:154-157) of frame a (h, w) to roi = (x, y, w, h): roi.x + x in 32 bits, gs_get's
-    0 outside the frame.  The caller has checked the assert."""
-    h, w = a.shape
-    x, y, rw, rh = (int(v) for v in roi)
-    cx = (x + np.arange(rw, dtype=np.int64)) & M32
-    cy = (y + np.arange(rh, dtype=np.int64)) & M32
-    out = np.zeros((rh, rw), np.uint8)
-    vx, vy = cx < w, cy < h
-    out[np.ix_(vy, vx)] = a[np.ix_(cy[vy], cx[vx])]
-    return out
-
-
-def gso_resize_nn(c, dw, dh):
-    """gs_resize_nn (reference grayskull.h:164-169): x * src.w / dst.w in 32 bits"""
-    h, w = c.shape
-    sx = ((np.arange(dw, dtype=np.int64) * w) & M32) // max(dw, 1)
-    sy = ((np.arange(dh, dtype=np.int64) * h) & M32) // max(dh, 1)
-    out = np.zeros((dh, dw), np.uint8)
-    vx, vy = sx < w, sy < h
-    out[np.ix_(vy, vx)] = c[np.ix_(sy[vy], sx[vx])]
-    return out
-
-
-def roi_valid(roi, sw, sh):
-    x, y, w, h = (int(v) for v in roi)
-    return w > 0 and h > 0 and (x + w) & M32 <= sw and (y + h) & M32 <= sh
-
-
-def composition(Od, a, roi, dw, dh, mode):
-    """gs_crop then gs_resize_nn / gs_resize, one frame; an invalid region gives zeros (the device lists' rule)"""
-    if not roi_valid(roi, a.shape[1], a.shape[0]):
-        return np.zeros((dh, dw), np.uint8)
-    c = gso_crop(a, roi)
-    return gso_resize_nn(c, dw, dh) if mode == NEAREST else L.o_resize(Od, np.ascontiguousarray(c), dw, dh)
 
 
 def roi_lib():
