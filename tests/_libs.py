@@ -493,6 +493,24 @@ def composition(Od, a, roi, dw, dh, mode):
     return gso_resize_nn(c, dw, dh) if mode == 0 else o_resize(Od, np.ascontiguousarray(c), dw, dh)
 
 
+def regions(rng, n, max_rects, sw, sh, dw, dh, invalid=True):
+    """(n, max_rects) regions of a sw x sh frame: every fourth one unscaled to dw x dh (a copy slot), the rest random;
+    with `invalid`, some that gs_crop's assert would reject"""
+    r = np.zeros((n, max_rects), RECT_DTYPE)
+    for f in range(n):
+        for k in range(max_rects):
+            kind = k % 4
+            if kind == 0:                                   # unscaled: a copy slot
+                w, h = dw, dh
+            else:
+                w, h = int(rng.integers(1, sw + 1)), int(rng.integers(1, sh + 1))
+            x, y = int(rng.integers(0, sw - w + 1)) if w <= sw else 0, int(rng.integers(0, sh - h + 1)) if h <= sh else 0
+            if invalid and kind == 3 and k % 8 == 3:        # gs_crop's assert would reject these: zero slots
+                x, y, w, h = [(sw - w + 1, y, w, h), (x, y, 0, h), (x, y, w, 0), (x, sh, w, h)][(f + k) % 4]
+            r[f, k] = (x, y, w, h)
+    return r
+
+
 # ---- the reference CLI's pyramid ORB, restated (tests/test_orb_pyramid.py) ---------------------------------------------
 def level_rule(w, h, levels):
     """nanomagick.c:247,255-260: min(levels, 4) levels, stopping before one with w/2 < 32 or h/2 < 32"""

@@ -36,10 +36,11 @@ import re
 import numpy as np
 import pytest
 
+import _calls as calls
 import _libs as L
 from _gpu import O, lib, stream, traced, witness, witnessed  # noqa: F401
 
-POISON = 0xA5
+POISON = calls.POISON
 GUARD = 64
 NS = (65535, 65536, 2 * 65535 + 3)
 W, H = 48, 40
@@ -119,7 +120,7 @@ def test_every_batch_entry_point_has_a_row():
     assert len(ids) == len(set(ids))
 
 
-# ---- per-row specs: distinct frames -> inputs and expected outputs (bytes per frame) ----------------------------------
+# ---- per-row inputs: the distinct frames and their per-frame inputs ------------------------------------------------
 def _frames7(w, h, seed):
     rng = np.random.default_rng(seed)
     out = [rng.integers(0, 256, (h, w), dtype=np.uint8), L.natural_like(w, h, seed), np.full((h, w), 255, np.uint8),
@@ -128,232 +129,53 @@ def _frames7(w, h, seed):
     return np.stack(out)
 
 
-def _records(lists, cap, dtype):
-    """per frame: its records, then poison up to cap slots -> (k, cap * itemsize) bytes"""
-    out = np.full((len(lists), cap * dtype.itemsize), POISON, np.uint8)
-    for i, r in enumerate(lists):
-        b = np.ascontiguousarray(r).view(np.uint8).reshape(-1)
-        out[i, :b.size] = b
-    return out
-
-
-def _counts(lists):
-    return np.array([[len(r)] for r in lists], np.uint32).view(np.uint8)
-
-
-def _box(O, g, fr, adaptive):
-    if adaptive:
-        return {"dst": np.stack([L.o_adaptive(O, a, g["r"], g["c"]) for a in fr])}
-    return {"dst": np.stack([L.o_blur(O, a, g["r"]) for a in fr])}
-
-
-def _morph_n(O, fr, dil, iters):
-    out = []
-    for a in fr:
-        for _ in range(iters):
-            a = L.o_morph(O, a, dil)
-        out.append(a)
-    return np.stack(out)
-
-
-def _fast(O, g, fr, orb):
-    sms, lists = [], []
-    for a in fr:
-        sm = np.full_like(a, POISON)
-        lists.append(L.o_orb(O, a, sm, g["nkps"], g["t"]) if orb else L.o_fast(O, a, sm, g["nkps"], g["t"]))
-        sms.append(sm)
-    return {"scoremap": np.stack(sms), "kps": _records(lists, g["nkps"], L.KP_DTYPE), "counts": _counts(lists)}
-
-
-def _o_blobs(O, a, nb):
-    h, w = a.shape
-    labels, blobs = np.zeros((h, w), np.uint16), np.zeros(nb, L.BLOB_DTYPE)
-    m = O.gso_blobs(L.ptr(a), w, h, L.ptr(labels), L.ptr(blobs), nb)
-    return labels, blobs[:m]
-
-
 def _lbp_frames(w, h):
-    lena = np.load(os.path.join(L.ROOT, "tests", "golden", "lena_golden.npz"))["lena"]
     at = [(44, 40), (0, 0), (48, 44), (52, 44), (20, 10), (40, 40), (64, 64)]
-    return np.stack([np.ascontiguousarray(lena[y:y + h, x:x + w]) for x, y in at])
+    return np.stack([np.ascontiguousarray(calls.lena()[y:y + h, x:x + w]) for x, y in at])
 
 
-def spec(lib, O, sym, g, fr=None):
-    """-> (inputs, outputs, call): inputs / outputs map a buffer name to the per-frame bytes of each distinct frame
-    (outputs: what the call must leave there, poison where it writes nothing); a list of such arrays is a buffer whose
-    segments each hold n frames (level-major layouts).  call(P, n) makes the C call on the buffers' device pointers."""
+def row_inputs(O, sym, g, fr=None):
+    """{buffer: its bytes for each distinct frame}: fr, else the period-7 frames, and the row's per-frame inputs"""
     w, h = g["w"], g["h"]
-    if fr is None and sym != "match_orb":
-        fr = _frames7(w, h, w * 7 + h)
-    k = 7 if fr is None else len(fr)
-    s = stream()
-    if sym in ("blur", "adaptive_threshold"):
-        ad = sym != "blur"
-        fn = (lambda P, n: lib.gs_b200_adaptive_threshold_batch(P["dst"], P["src"], w, h, n, g["r"], g["c"], s)) if ad else (
-            lambda P, n: lib.gs_b200_blur_batch(P["dst"], P["src"], w, h, n, g["r"], s))
-        return {"src": fr}, _box(O, g, fr, ad), fn
-    if sym in ("sobel", "erode", "dilate"):
-        if sym == "sobel":
-            want = np.stack([L.o_sobel(O, a, POISON) for a in fr])
-        else:
-            want = np.stack([L.o_morph(O, a, sym == "dilate") for a in fr])
-        f = getattr(lib, "gs_b200_%s_batch" % sym)
-        return {"src": fr}, {"dst": want}, lambda P, n: f(P["dst"], P["src"], w, h, n, s)
-    if sym == "blur_sobel":
-        want = np.stack([L.o_sobel(O, L.o_blur(O, a, g["r"]), POISON) for a in fr])
-        return {"src": fr}, {"dst": want}, lambda P, n: lib.gs_b200_blur_sobel_batch(P["dst"], P["src"], w, h, n, g["r"], s)
-    if sym in ("erode_n", "dilate_n"):
-        f = getattr(lib, "gs_b200_%s_batch" % sym)
-        return {"src": fr}, {"dst": _morph_n(O, fr, sym == "dilate_n", g["iters"])}, \
-            lambda P, n: f(P["dst"], P["src"], w, h, n, g["iters"], s)
-    if sym == "resize":
-        want = np.stack([L.o_resize(O, a, g["dw"], g["dh"]) for a in fr])
-        return {"src": fr}, {"dst": want}, lambda P, n: lib.gs_b200_resize_batch(P["dst"], g["dw"], g["dh"], P["src"], w, h, n, s)
-    if sym == "downsample":
-        return {"src": fr}, {"dst": np.stack([L.o_down(O, a) for a in fr])}, \
-            lambda P, n: lib.gs_b200_downsample_batch(P["dst"], P["src"], w, h, n, s)
-    if sym == "integral":
-        return {"src": fr}, {"ii": np.stack([L.o_integral(O, a) for a in fr])}, \
-            lambda P, n: lib.gs_b200_integral_batch(P["ii"], P["src"], w, h, n, s)
-    if sym == "histogram":
-        want = np.stack([np.bincount(a.ravel(), minlength=256).astype(np.uint32) for a in fr])
-        return {"src": fr}, {"hist": want}, lambda P, n: lib.gs_b200_histogram_batch(P["hist"], P["src"], w, h, n, s)
-    if sym == "otsu_threshold":
-        hist = np.stack([np.bincount(a.ravel(), minlength=256).astype(np.uint32) for a in fr])
-        thr = np.array([[O.gso_otsu_threshold(L.ptr(a), w, h)] for a in fr], np.uint8)
-        return {"src": fr}, {"thresh": thr, "hist": hist}, \
-            lambda P, n: lib.gs_b200_otsu_threshold_batch(P["thresh"], P["hist"], P["src"], w, h, n, s)
-    if sym in ("threshold", "threshold_each"):
-        thr = np.array([[100], [0], [250], [37], [255], [128], [1]], np.uint8)[:k] if sym == "threshold_each" else None
-        want = []
-        for i, a in enumerate(fr):
-            b = a.copy()
-            O.gso_threshold(L.ptr(b), w, h, g["t"] if thr is None else (int(thr[i, 0]) + g["offset"]) & 255)
-            want.append(b)
-        if thr is None:
-            return {"img": fr}, {"img": np.stack(want)}, lambda P, n: lib.gs_b200_threshold_batch(P["img"], w, h, n, g["t"], s)
-        return {"img": fr, "thresh": thr}, {"img": np.stack(want)}, \
-            lambda P, n: lib.gs_b200_threshold_each_batch(P["img"], w, h, n, P["thresh"], g["offset"], s)
-    if sym == "filter":
-        ks, norm = L.filter_kernel(g["k"])
-        ks = np.ascontiguousarray(ks)
-        want = []
-        for a in fr:
-            d = np.zeros_like(a)
-            O.gso_filter(L.ptr(d), L.ptr(a), w, h, L.ptr(ks), ks.shape[1], ks.shape[0], norm)
-            want.append(d)
-        return {"src": fr}, {"dst": np.stack(want)}, lambda P, n: lib.gs_b200_filter_batch(
-            P["dst"], P["src"], w, h, n, ks.ctypes.data, ks.shape[1], ks.shape[0], norm, s)
-    if sym == "match_template":
-        tw, th = g["tw"], g["th"]
-        tmpl = np.ascontiguousarray(_frames7(w, h, w * 7 + h)[1, 10:10 + th, 20:20 + tw])
-        T = dev_buf(tmpl)
-        rw, rh = w - tw + 1, h - th + 1
-        want = []
-        for a in fr:
-            d = np.zeros((rh, rw), np.uint8)
-            O.gso_match_template(L.ptr(a), w, h, L.ptr(tmpl), tw, th, L.ptr(d))
-            want.append(d)
-        return {"img": fr}, {"result": np.stack(want)}, lambda P, n: lib.gs_b200_match_template_batch(
-            P["result"], P["img"], w, h, n, T.data_ptr(), tw, th, s)
-    if sym == "find_best_match":
-        maps = (fr // 2).astype(np.uint8)                      # a result map per frame, the 255 frame -> all ties
-        best = []
-        for a in maps:
-            b = O.gso_find_best_match(L.ptr(np.ascontiguousarray(a)), w, h)
-            best.append([b % w, b // w])
-        return {"result": maps}, {"best": np.array(best, np.uint32)}, \
-            lambda P, n: lib.gs_b200_find_best_match_batch(P["best"], P["result"], w, h, n, s)
-    if sym == "blobs":
-        nb = g["nb"]
-        if g.get("binary", True):
-            fr = np.stack([L.binary_like(w, h, 50 + i) if i % 3 else np.where(a >= 128, 255, 0).astype(np.uint8)
-                           for i, a in enumerate(fr)]) if len(fr) == 7 else fr
-        res = [_o_blobs(O, a, nb) for a in fr]
-        return {"img": fr}, {"labels": np.stack([lb for lb, _ in res]), "blobs": _records([b for _, b in res], nb, L.BLOB_DTYPE),
-                             "counts": _counts([b for _, b in res])}, \
-            lambda P, n: lib.gs_b200_blobs_batch(P["img"], w, h, n, P["labels"], P["blobs"], P["counts"], nb, s)
-    if sym == "perspective_correct":
-        dw, dh = g["dw"], g["dh"]
-        quads = np.random.default_rng(5).integers(0, min(w, h), (k, 4, 2)).astype(np.uint32)
-        want = []
-        for a, q in zip(fr, quads):
-            d = np.empty((dh, dw), np.uint8)
-            O.gso_perspective_correct(L.ptr(d), dw, dh, L.ptr(a), w, h, L.ptr(np.ascontiguousarray(q)))
-            want.append(d)
-        return {"src": fr, "corners": quads}, {"dst": np.stack(want)}, lambda P, n: lib.gs_b200_perspective_correct_batch(
-            P["dst"], dw, dh, P["src"], w, h, n, P["corners"], 1, s)
-    if sym in ("fast", "orb_extract"):
-        orb = sym == "orb_extract"
-        f = lib.gs_b200_orb_extract_batch if orb else lib.gs_b200_fast_batch
-        return {"src": fr}, _fast(O, g, fr, orb), lambda P, n: f(P["src"], w, h, n, P["scoremap"], P["kps"], P["counts"],
-                                                                g["nkps"], g["t"], s)
     if sym == "match_orb":
-        s1, s2, mm = g["s1"], g["s2"], g["mm"]
         rng = np.random.default_rng(16)
-        sizes = g.get("sizes", [(40, 30), (7, 0), (0, 12), (33, 29), (1, 1), (40, 2), (25, 30)])
-        sets = [L.desc_sets(rng, a, b) for a, b in sizes]
-        k1, k2 = np.zeros((len(sets), s1), L.KP_DTYPE), np.zeros((len(sets), s2), L.KP_DTYPE)
+        sets = [L.desc_sets(rng, a, b) for a, b in g.get("sizes", [(40, 30), (7, 0), (0, 12), (33, 29), (1, 1), (40, 2),
+                                                                    (25, 30)])]
+        k1, k2 = np.zeros((len(sets), g["s1"]), L.KP_DTYPE), np.zeros((len(sets), g["s2"]), L.KP_DTYPE)
         for i, (a, b) in enumerate(sets):
             k1[i, :len(a)], k2[i, :len(b)] = a, b
-        c1 = np.array([[len(a)] for a, _ in sets], np.uint32)
-        c2 = np.array([[len(b)] for _, b in sets], np.uint32)
-        lists = [L.o_match(O, a, b, mm, 60.0) for a, b in sets]
-        return {"kps1": k1, "n1": c1, "kps2": k2, "n2": c2}, \
-            {"matches": _records(lists, mm, L.MATCH_DTYPE), "counts": _counts(lists)}, \
-            lambda P, n: lib.gs_b200_match_orb_batch(P["kps1"], P["n1"], s1, P["kps2"], P["n2"], s2, n, P["matches"],
-                                                      P["counts"], mm, 60.0, s)
+        return {"kps1": k1, "n1": calls.counts([a for a, _ in sets]), "kps2": k2, "n2": calls.counts([b for _, b in sets])}
     if sym == "lbp_detect":
-        import grayskull_b200 as gb
-        cas = gb.load_cascade()
-        mr = g["mr"]
-        if g.get("lena", True):
-            fr = _lbp_frames(w, h)
-        ii = np.stack([L.o_integral(O, a) for a in fr])
-        lists = [L.o_detect(O, cas, t, mr, 1.1, 1.0, 4.0, 2) for t in ii]
-        assert sum(len(r) for r in lists) > 0 and min(len(r) for r in lists) == 0
-        return {"ii": ii}, {"rects": _records(lists, mr, L.RECT_DTYPE), "counts": _counts(lists)}, \
-            lambda P, n: lib.gs_b200_lbp_detect_batch(cas.ptr, P["ii"], w, h, n, P["rects"], P["counts"], mr, 1.1, 1.0, 4.0,
-                                                       2, s)
-    if sym in ("crop_resize", "rois_resize"):
-        dw, dh = g["dw"], g["dh"]
-        if sym == "crop_resize":
-            from grayskull_b200._lib import Rect
-            roi = g["roi"]
-            want = np.stack([L.composition(O, a, roi, dw, dh, 1) for a in fr])
-            return {"src": fr}, {"dst": want}, lambda P, n: lib.gs_b200_crop_resize_batch(
-                P["dst"], dw, dh, P["src"], w, h, n, Rect(*roi), 1, s)
-        mr = g["mr"]
+        return {"ii": np.stack([L.o_integral(O, a) for a in _lbp_frames(w, h)])}
+    fr = _frames7(w, h, w * 7 + h) if fr is None else fr
+    k = len(fr)
+    if sym == "threshold_each":
+        return {"src": fr, "thresh": np.array([100, 0, 250, 37, 255, 128, 1], np.uint8)[:k]}
+    if sym == "match_template":
+        return {"src": fr, "tmpl": np.ascontiguousarray(_frames7(w, h, w * 7 + h)[1, 10:10 + g["th"], 20:20 + g["tw"]])}
+    if sym == "find_best_match":
+        return {"res": (fr // 2).astype(np.uint8)}                    # a result map per frame, the 255 frame -> all ties
+    if sym == "blobs" and g.get("binary", True):
+        return {"src": np.stack([L.binary_like(w, h, 50 + i) if i % 3 else np.where(a >= 128, 255, 0).astype(np.uint8)
+                                 for i, a in enumerate(fr)])}
+    if sym == "perspective_correct":
+        return {"src": fr, "corners": np.random.default_rng(5).integers(0, min(w, h), (k, 4, 2)).astype(np.uint32)}
+    if sym in ("fast", "orb_extract"):
+        return {"src": fr, "score": np.full_like(fr, POISON)}
+    if sym == "rois_resize":
+        dw, dh, mr = g["dw"], g["dh"], g["mr"]
         rng = np.random.default_rng(3)
         rects = np.zeros((k, mr), L.RECT_DTYPE)
         for i in range(k):
             for j in range(mr):
                 rw, rh = (dw, dh) if j == 0 else (int(rng.integers(1, w)), int(rng.integers(1, h)))
                 rects[i, j] = (int(rng.integers(0, w - rw + 1)), int(rng.integers(0, h - rh + 1)), rw, rh)
-        cnt = np.array([[(3 + i) % (mr + 1)] for i in range(k)], np.uint32)
-        want = np.full((k, mr, dh, dw), POISON, np.uint8)
-        for i in range(k):
-            for j in range(int(cnt[i, 0])):
-                want[i, j] = L.composition(O, fr[i], tuple(rects[i, j]), dw, dh, 1)
-        return {"src": fr, "rects": rects, "rcounts": cnt}, {"dst": want}, lambda P, n: lib.gs_b200_rois_resize_batch(
-            P["dst"], dw, dh, P["src"], w, h, n, P["rects"], P["rcounts"], mr, 1, s)
+        return {"src": fr, "rects": rects, "rcounts": np.array([(3 + i) % (mr + 1) for i in range(k)], np.uint32)}
     if sym == "orb_pyramid":
-        nkps, t, lv = g["nkps"], g["t"], g["levels"]
-        sizes = L.layout(w, h, lv)[0]
+        sizes = L.layout(w, h, g["levels"])[0]
         assert len(sizes) == 2
-        maps0 = np.full(sum(a * b for a, b in sizes) * k, POISON, np.uint8)
-        kl, pyr, maps = L.pyramid_expected(O, fr, nkps, t, lv, maps0)
-        b0 = w * h * k
-        return {"src": fr}, {"pyr": pyr.reshape(k, -1), "scoremap": [maps[:b0].reshape(k, -1), maps[b0:].reshape(k, -1)],
-                             "kps": _records(kl, nkps, L.KP_DTYPE), "counts": _counts(kl)}, \
-            lambda P, n: lib.gs_b200_orb_pyramid_batch(P["src"], w, h, n, lv, P["pyr"], P["scoremap"], P["kps"], P["counts"],
-                                                       nkps, t, s)
-    raise KeyError(sym)
-
-
-def dev_buf(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a).reshape(-1).view(np.uint8).copy()).cuda()
+        return {"src": fr, "score": [np.full((k, a * b), POISON, np.uint8) for a, b in sizes]}
+    return {"src": fr}
 
 
 def _chunk(per):
@@ -364,13 +186,12 @@ def _chunk(per):
 class Batch:
     """a device buffer of n frames of `per` bytes (or level-major segments of such), plus GUARD poison bytes after it"""
 
-    def __init__(self, segs, n, idx, src=None):
+    def __init__(self, segs, n, idx, src=False):
         import torch
-        self.segs = [np.ascontiguousarray(x).reshape(len(x), -1).view(np.uint8) for x in segs]
-        self.n = n
+        self.segs, self.n = segs, n
         size = sum(n * x.shape[1] for x in self.segs)
         self.t = torch.full((size + GUARD,), POISON, dtype=torch.uint8, device="cuda")
-        if src is not None:                              # an input: frame f holds distinct frame idx[f]
+        if src:                                          # an input: frame f holds distinct frame idx[f]
             off = 0
             for x in self.segs:
                 d, per = torch.from_numpy(x.copy()).cuda(), x.shape[1]
@@ -405,18 +226,22 @@ def run_batch(lib, O, sym, g, n, idx, fr=None):
     import torch
     free0 = torch.cuda.mem_get_info()[0]
     torch.cuda.reset_peak_memory_stats()
-    ins, outs, call = spec(lib, O, sym, g, fr)
-    bufs = {k: Batch(v if isinstance(v, list) else [v], n, idx, src=True) for k, v in ins.items()}
-    for k, v in outs.items():
-        if k not in bufs:
-            bufs[k] = Batch(v if isinstance(v, list) else [v], n, idx)
-    rc, seen = traced(lambda: call({k: b.ptr for k, b in bufs.items()}, n))
+    sp, ins = calls.spec("gs_b200_%s_batch" % sym, g), row_inputs(O, sym, g, fr)
+    k = len(next(iter(ins.values())))                  # the first buffer is per frame and not segmented
+    before = calls.filled(sp, k)
+    want = sp.expect(ins, before)
+    if sym == "lbp_detect":
+        assert want["counts"].sum() > 0 and want["counts"].min() == 0
+    shared = {b: torch.from_numpy(calls.flat(ins[b], 1)).cuda() for b in sp.shared}
+    bufs = {b: Batch(calls.segments(x, k), n, idx, src=True) for b, x in ins.items() if b not in sp.shared}
+    bufs.update({b: Batch(calls.segments(x, k), n, idx) for b, x in before.items()})
+    P = dict({b: t.data_ptr() for b, t in shared.items()}, **{b: x.ptr for b, x in bufs.items()})
+    rc, seen = traced(lambda: sp.call(P, n, stream()))
     assert rc == 0, lib.gs_b200_last_error().decode()
-    for k, b in bufs.items():
-        if k in outs:
-            b.segs = [np.ascontiguousarray(x).reshape(len(x), -1).view(np.uint8)
-                      for x in (outs[k] if isinstance(outs[k], list) else [outs[k]])]
-        b.check(k, idx)
+    for b, x in bufs.items():
+        if b in want:
+            x.segs = calls.segments(want[b], k)
+        x.check(b, idx)
     took = free0 - torch.cuda.mem_get_info()[0]
     print("\n%s n=%d: device memory taken %.2f GB (torch peak %.2f GB)" %
           (sym, n, took / 1e9, torch.cuda.max_memory_allocated() / 1e9))

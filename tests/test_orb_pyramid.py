@@ -14,25 +14,25 @@ test_dispatch_paths.py that its launches go through gsb::launch.
   * GPU: every frame bit-exact against the restatement -- keypoints up to the count, untouched slots after it, every
     pyramid byte and every score-map byte with the caller's bytes as the maps' start -- at tiled and generic widths,
     L = 1..4 and a request for 5, skipped early levels, corner-rich frames whose last level's per-frame cap truncates,
-    trig mode 1, n = 0 and nkps = 0; the CLI's orb stage against the compiled reference CLI; ordering on the caller's
-    stream, two streams at once, graph capture with replay on new inputs, and refused workspace growth under capture.
+    trig mode 1, n = 0 and nkps = 0; the CLI's orb stage against the compiled reference CLI.  test_streams.py
+    runs the call on the caller's stream, on two streams at once, in a graph, and refuses its workspace growth under
+    capture.
 """
 import ctypes as C
 import os
 import re
 import subprocess
 import sys
-import time
 
 import numpy as np
 import pytest
 
 import _libs as L
+from _calls import POISON
 from _libs import layout, level_rule, pyramid_orb
 from _gpu import O, frames, lib, traced, witness, witnessed  # noqa: F401
 
 ROOT = L.ROOT
-POISON = 0xCD
 QUOTA, MERGE = "gsb::k_pyr_quota", "gsb::k_pyr_merge"
 FAST_T, FAST_G = "gsb::k_fast_tiled2<true>", "gsb::k_fast_tiled2<false>"   # TMA tile loads, or plain loads
 SELECT, BRIEF_W, BRIEF_B = "gsb::k_orb_select", "gsb::k_orb_brief<true>", "gsb::k_orb_brief<false>"
@@ -327,147 +327,3 @@ def test_gsb_magick_orb_stage(lib, O, tmp_path, pair):
         assert lines[f] == "frame %d: %s" % (f, want), (lines, want)
         data = (tmp_path / ("out%04d.pgm" % f)).read_bytes()
         assert data[-s.size:] == s.tobytes(), "frame %d changed" % f
-
-
-# ---- GPU: streams ---------------------------------------------------------------------------------------------------------
-SLEEP_CYCLES = 100_000_000           # ~50 ms at 1.98 GHz
-
-
-class StreamRun:
-    """one pyramid call on a stream, with its inputs staged on that stream"""
-
-    def __init__(self, n=3, w=320, h=240, nkps=600, levels=3):
-        import torch
-        self.n, self.w, self.h, self.nkps, self.levels = n, w, h, nkps, levels
-        self.sizes = layout(w, h, levels)[0]
-        self.nmaps = sum(a * b for a, b in self.sizes) * n
-        self.below = sum(a * b for a, b in self.sizes[1:]) * n
-        self.data = {seed: frames(w, h, n, 40 + seed) for seed in (1, 2)}
-        self.maps0 = {seed: np.random.default_rng(seed).integers(0, 256, self.nmaps, dtype=np.uint8) for seed in (1, 2)}
-        self.dev = {seed: torch.from_numpy(a).cuda() for seed, a in self.data.items()}
-        self.dmaps = {seed: torch.from_numpy(m).cuda() for seed, m in self.maps0.items()}
-        self.src = torch.empty_like(self.dev[1])
-        self.sm = torch.empty(self.nmaps, dtype=torch.uint8, device="cuda")
-        self.pyr = torch.empty(max(self.below, 1), dtype=torch.uint8, device="cuda")
-        self.kps = torch.empty((n, nkps, 48), dtype=torch.uint8, device="cuda")
-        self.counts = torch.empty(n, dtype=torch.int32, device="cuda")
-        torch.cuda.synchronize()
-
-    def stage(self, s, seed):
-        import torch
-        with torch.cuda.stream(s):
-            self.src.copy_(self.dev[seed], non_blocking=True)
-            self.sm.copy_(self.dmaps[seed], non_blocking=True)
-            self.kps.fill_(POISON)
-
-    def call(self, s):
-        return pyramid_lib().gs_b200_orb_pyramid_batch(self.src.data_ptr(), self.w, self.h, self.n, self.levels,
-                                                       self.pyr.data_ptr(), self.sm.data_ptr(), self.kps.data_ptr(),
-                                                       self.counts.data_ptr(), self.nkps, 20, C.c_void_p(s.cuda_stream))
-
-    def grab(self, s):
-        import torch
-        with torch.cuda.stream(s):
-            return self.counts.clone(), self.kps.clone(), self.pyr.clone(), self.sm.clone()
-
-    def verify(self, got, seed):
-        counts, kps, pyr, sm = (t.cpu().numpy() for t in got)
-        c = dict(nkps=self.nkps, trig=0)
-        want = L.pyramid_expected(L.oracle(), self.data[seed], self.nkps, 20, self.levels, self.maps0[seed])
-        _check(c, counts, kps, pyr[:self.below], sm, want)
-
-
-def _sleep(s, cycles):
-    import torch
-    with torch.cuda.stream(s):
-        torch.cuda._sleep(int(cycles))
-
-
-def _ok(rc):
-    from grayskull_b200 import _lib
-    _lib.check(rc, "orb_pyramid_batch")
-
-
-@pytest.mark.gpu
-def test_ordered_and_asynchronous(lib):
-    import torch
-    run, s, u = StreamRun(), torch.cuda.Stream(), torch.cuda.Stream()
-    run.stage(s, 2)
-    _ok(run.call(s))
-    s.synchronize()
-    run.verify(run.grab(s), 2)
-    _sleep(u, 2 * SLEEP_CYCLES)
-    _sleep(s, SLEEP_CYCLES)
-    run.stage(s, 1)
-    t0 = time.perf_counter()
-    rc = run.call(s)
-    host = time.perf_counter() - t0
-    s_done, u_done = s.query(), u.query()
-    got = run.grab(s)
-    torch.cuda.synchronize()
-    _ok(rc)
-    assert not s_done, "returned after its stream had drained (host time %.1f ms): it waited for it" % (host * 1e3)
-    assert not u_done, "returned after another stream had drained: it synchronised the device"
-    run.verify(got, 1)
-
-
-@pytest.mark.gpu
-def test_two_streams_at_once(lib):
-    import torch
-    s0, s1 = torch.cuda.Stream(), torch.cuda.Stream()
-    r0, r1 = StreamRun(), StreamRun(n=2, w=264, h=131, nkps=301, levels=4)
-    _sleep(s1, SLEEP_CYCLES // 2)
-    got = []
-    for r, s in ((r0, s0), (r1, s1)):
-        r.stage(s, 1)
-        _ok(r.call(s))
-        got.append((r, r.grab(s)))
-    torch.cuda.synchronize()
-    for r, g in got:
-        r.verify(g, 1)
-
-
-@pytest.mark.gpu
-def test_graph_capture_and_replay(lib):
-    import torch
-    run, s = StreamRun(), torch.cuda.Stream()
-    run.stage(s, 2)
-    _ok(run.call(s))
-    s.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g, stream=s):
-        rc = run.call(s)
-    _ok(rc)
-    for seed in (1, 2):
-        run.stage(s, seed)
-        with torch.cuda.stream(s):
-            g.replay()
-        got = run.grab(s)
-        s.synchronize()
-        run.verify(got, seed)
-
-
-@pytest.mark.gpu
-def test_capture_that_would_grow_the_workspace_is_refused(lib):
-    import torch
-    small, s = StreamRun(n=1, w=128, h=96, nkps=50), torch.cuda.Stream()
-    small.stage(s, 1)
-    _ok(small.call(s))
-    s.synchronize()
-    big = StreamRun(n=3, w=512, h=384, nkps=2000)
-    big.stage(s, 1)
-    s.synchronize()
-    g = torch.cuda.CUDAGraph()
-    rc = None
-    try:
-        with torch.cuda.graph(g, stream=s):
-            rc = big.call(s)
-    except RuntimeError:
-        pass                       # torch reports the empty / invalidated capture; the call's status is what counts
-    assert rc == 900, (rc, lib.gs_b200_last_error())     # cudaErrorStreamCaptureUnsupported
-    assert b"capturing" in lib.gs_b200_last_error()
-    torch.cuda.synchronize()
-    big.stage(s, 2)                # outside a capture the same call grows its workspace and runs
-    _ok(big.call(s))
-    s.synchronize()
-    big.verify(big.grab(s), 2)

@@ -13,25 +13,24 @@ test_dispatch_paths.py that its launches go through gsb::launch.
   * GPU: both entry points against the composition (host regions at TMA-friendly and ragged widths, odd offsets,
     misaligned pointers; device lists with and without counts, untouched slots past the counts, invalid regions,
     a source batch over 4 GiB); LBP detection chained into the region call on the device counts; the CLI's crop
-    stage; ordering on the caller's stream, two streams at once, and graph capture with replay on new inputs.
+    stage.  test_streams.py runs both entry points on the caller's stream, on two streams at once and in a graph.
 """
 import ctypes as C
 import os
 import subprocess
 import sys
-import time
 
 import numpy as np
 import pytest
 
 import _libs as L
+from _calls import POISON
 from _libs import M32, composition, gso_crop, gso_resize_nn, roi_valid  # noqa: F401
 from grayskull_b200._lib import Rect
 from _gpu import O, Region, frames, lib, stream, traced, witness, witnessed  # noqa: F401
 
 ROOT = L.ROOT
 NEAREST, BILINEAR = 0, 1
-FILL = 0xA5
 COPY, NN, BL = "gsb::k_roi_copy", "gsb::k_roi_gather<0>", "gsb::k_roi_gather<1>"
 # kernel -> the cases of this file that must launch it (test ids), checked by the census below
 DISPATCH = {
@@ -215,22 +214,6 @@ def test_whole_frame_bilinear_equals_resize_batch(lib, geom):
 
 
 # ---- GPU: region lists ---------------------------------------------------------------------------------------------------
-def _regions(rng, n, max_rects, sw, sh, dw, dh, invalid=True):
-    r = np.zeros((n, max_rects), L.RECT_DTYPE)
-    for f in range(n):
-        for k in range(max_rects):
-            kind = k % 4
-            if kind == 0:                                   # unscaled: a copy slot
-                w, h = dw, dh
-            else:
-                w, h = int(rng.integers(1, sw + 1)), int(rng.integers(1, sh + 1))
-            x, y = int(rng.integers(0, sw - w + 1)) if w <= sw else 0, int(rng.integers(0, sh - h + 1)) if h <= sh else 0
-            if invalid and kind == 3 and k % 8 == 3:        # gs_crop's assert would reject these: zero slots
-                x, y, w, h = [(sw - w + 1, y, w, h), (x, y, 0, h), (x, y, w, 0), (x, sh, w, h)][(f + k) % 4]
-            r[f, k] = (x, y, w, h)
-    return r
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode", [NEAREST, BILINEAR], ids=["nearest", "bilinear"])
 @pytest.mark.parametrize("counts", ["null", "partial"])
@@ -242,7 +225,7 @@ def test_rois_resize_vs_oracle(lib, O, witness, mode, counts, geom):
     n, mr = 4, 8
     rng = np.random.default_rng(sw + 7 * mode)
     a = frames(sw, sh, n, 5)
-    rects = _regions(rng, n, mr, sw, sh, dw, dh)
+    rects = L.regions(rng, n, mr, sw, sh, dw, dh)
     cnt = np.array([mr, 3, 0, 5 + 2 * mode], np.uint32) if counts == "partial" else None
     src = Region(a.nbytes, so, a, 1)
     dst = Region(n * mr * dw * dh, do, seed=2)
@@ -284,12 +267,12 @@ def test_rois_in_the_last_frame_of_a_batch_over_4gib(lib, O):
     R = torch.from_numpy(rects.view(np.int32).reshape(n, 3, 4)).cuda()
     N = torch.from_numpy(cnt).cuda()
     for mode in (NEAREST, BILINEAR):
-        out = torch.full((n, 3, 64, 64), FILL, dtype=torch.uint8, device="cuda")
+        out = torch.full((n, 3, 64, 64), POISON, dtype=torch.uint8, device="cuda")
         roi.rois_resize_batch(src, R, N, 64, 64, mode, out=out)
         got = out[n - 1].cpu().numpy()
         for k in range(3):
             assert np.array_equal(got[k], composition(O, last, tuple(rects[n - 1, k]), 64, 64, mode)), (mode, k)
-        assert bool((out[: n - 1] == FILL).all()), "slots of frames with count 0 changed"
+        assert bool((out[: n - 1] == POISON).all()), "slots of frames with count 0 changed"
     del src
     torch.cuda.empty_cache()
 
@@ -308,7 +291,7 @@ def test_lbp_detect_into_rois(lib, O, mode):
     mr = 32
     src = torch.from_numpy(fr).cuda()
     rects, counts = api.lbp_detect_batch(cas, api.integral_batch(src), mr, 1.1, 1.0, 4.0, 2)
-    out = torch.full((n, mr, 24, 24), FILL, dtype=torch.uint8, device="cuda")
+    out = torch.full((n, mr, 24, 24), POISON, dtype=torch.uint8, device="cuda")
     roi.rois_resize_batch(src, rects, counts, 24, 24, mode, out=out)
     got = out.cpu().numpy()
     total = 0
@@ -318,7 +301,7 @@ def test_lbp_detect_into_rois(lib, O, mode):
         total += len(want_rects)
         for k, r in enumerate(want_rects):
             assert np.array_equal(got[f, k], composition(O, fr[f], tuple(r), 24, 24, mode)), (f, k, r)
-        assert (got[f, len(want_rects):] == FILL).all()
+        assert (got[f, len(want_rects):] == POISON).all()
     assert total > 0, "no detections: the chain was not exercised"
 
 
@@ -345,138 +328,3 @@ def test_gsb_magick_crop_stage(lib, tmp_path):
         assert np.array_equal(np.frombuffer(data[-61 * 37:], np.uint8).reshape(37, 61), want)
     r = subprocess.run([exe, "crop:100:0:30:5", str(tmp_path / "bad")] + ins, capture_output=True, text=True, timeout=120)
     assert r.returncode != 0 and "invalid crop rectangle" in r.stderr
-
-
-# ---- GPU: streams ---------------------------------------------------------------------------------------------------------
-SLEEP_CYCLES = 100_000_000           # ~50 ms at 1.98 GHz
-
-
-class StreamRun:
-    """one call of each entry point and mode on a stream, with its inputs staged on that stream"""
-
-    def __init__(self, entry, mode, n=3, sw=272, sh=70, dw=64, dh=48, mr=5):
-        import torch
-        self.entry, self.mode, self.n, self.sw, self.sh, self.dw, self.dh, self.mr = entry, mode, n, sw, sh, dw, dh, mr
-        self.data = {seed: frames(sw, sh, n, 40 + seed) for seed in (1, 2)}
-        self.dev = {seed: torch.from_numpy(a).cuda() for seed, a in self.data.items()}
-        self.src = torch.empty_like(self.dev[1])
-        rng = np.random.default_rng(mode)
-        self.rects = _regions(rng, n, mr, sw, sh, dw, dh, invalid=False)
-        self.rects[:, 0] = (5, 6, dw, dh)                    # a copy slot in each frame
-        self.roi = (9, 4, dw, dh) if mode == NEAREST else (9, 4, 80, 33)   # the copy kernel, then the gather one
-        self.R = torch.from_numpy(self.rects.view(np.int32).reshape(n, mr, 4)).cuda()
-        self.N = torch.from_numpy(np.array([mr, 2, 4][:n], np.int32)).cuda()
-        slots = n if entry == "host" else n * mr
-        self.out = torch.empty((slots, dh, dw), dtype=torch.uint8, device="cuda")
-        torch.cuda.synchronize()
-
-    def stage(self, s, seed):
-        import torch
-        with torch.cuda.stream(s):
-            self.src.copy_(self.dev[seed], non_blocking=True)
-            self.out.fill_(FILL)
-
-    def call(self, s):
-        from grayskull_b200 import roi
-        h = C.c_void_p(s.cuda_stream)
-        if self.entry == "host":
-            return roi.lib().gs_b200_crop_resize_batch(self.out.data_ptr(), self.dw, self.dh, self.src.data_ptr(),
-                                                       self.sw, self.sh, self.n, Rect(*self.roi), self.mode, h)
-        return roi.lib().gs_b200_rois_resize_batch(self.out.data_ptr(), self.dw, self.dh, self.src.data_ptr(), self.sw,
-                                                   self.sh, self.n, self.R.data_ptr(), self.N.data_ptr(), self.mr,
-                                                   self.mode, h)
-
-    def grab(self, s):
-        import torch
-        with torch.cuda.stream(s):
-            return self.out.clone()
-
-    def verify(self, got, seed):
-        Od = L.oracle()
-        got = got.cpu().numpy()
-        cnt = self.N.cpu().numpy()
-        for f in range(self.n):
-            a = self.data[seed][f]
-            if self.entry == "host":
-                assert np.array_equal(got[f], composition(Od, a, self.roi, self.dw, self.dh, self.mode)), f
-                continue
-            for k in range(self.mr):
-                want = composition(Od, a, tuple(self.rects[f, k]), self.dw, self.dh, self.mode) if k < cnt[f] else \
-                    np.full((self.dh, self.dw), FILL, np.uint8)
-                assert np.array_equal(got[f * self.mr + k], want), (seed, f, k)
-
-
-STREAM_ROWS = [pytest.param(e, m, id="%s-%s" % (e, ["nearest", "bilinear"][m])) for e in ("host", "list") for m in (0, 1)]
-
-
-def _sleep(s, cycles):
-    import torch
-    with torch.cuda.stream(s):
-        torch.cuda._sleep(int(cycles))
-
-
-def _ok(rc):
-    from grayskull_b200 import _lib
-    _lib.check(rc, "roi call")
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("entry,mode", STREAM_ROWS)
-def test_ordered_and_asynchronous(lib, entry, mode):
-    import torch
-    run, s, u = StreamRun(entry, mode), torch.cuda.Stream(), torch.cuda.Stream()
-    run.stage(s, 2)
-    _ok(run.call(s))
-    s.synchronize()
-    run.verify(run.out, 2)
-    _sleep(u, 2 * SLEEP_CYCLES)
-    _sleep(s, SLEEP_CYCLES)
-    run.stage(s, 1)
-    t0 = time.perf_counter()
-    rc = run.call(s)
-    host = time.perf_counter() - t0
-    s_done, u_done = s.query(), u.query()
-    got = run.grab(s)
-    torch.cuda.synchronize()
-    _ok(rc)
-    assert not s_done, "returned after its stream had drained (host time %.1f ms): it waited for it" % (host * 1e3)
-    assert not u_done, "returned after another stream had drained: it synchronised the device"
-    run.verify(got, 1)
-
-
-@pytest.mark.gpu
-def test_two_streams_at_once(lib):
-    import torch
-    s0, s1 = torch.cuda.Stream(), torch.cuda.Stream()
-    runs = [(StreamRun(e, m), StreamRun(e, m, n=2, sw=101, sh=37, dw=33, dh=20)) for e in ("host", "list") for m in (0, 1)]
-    _sleep(s1, SLEEP_CYCLES // 2)
-    got = []
-    for r0, r1 in runs:
-        for r, s in ((r0, s0), (r1, s1)):
-            r.stage(s, 1)
-            _ok(r.call(s))
-            got.append((r, r.grab(s)))
-    torch.cuda.synchronize()
-    for r, g in got:
-        r.verify(g, 1)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("entry,mode", STREAM_ROWS)
-def test_graph_capture_and_replay(lib, entry, mode):
-    import torch
-    run, s = StreamRun(entry, mode), torch.cuda.Stream()
-    run.stage(s, 2)
-    _ok(run.call(s))
-    s.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g, stream=s):
-        rc = run.call(s)
-    _ok(rc)
-    for seed in (1, 2):
-        run.stage(s, seed)
-        with torch.cuda.stream(s):
-            g.replay()
-        got = run.grab(s)
-        s.synchronize()
-        run.verify(got, seed)

@@ -2,11 +2,11 @@
 no hidden wait on the host, correct on two streams at once, on cudaStreamPerThread from two host threads, and inside a
 captured CUDA graph.
 
-CASES is the coverage record: one row per batch entry point of include/grayskull_b200.h that takes a gs_b200_stream,
-with a tiled and a generic geometry where the host code has both.  A row's spec gives its inputs for a seed, its
-outputs, the call on a stream and the oracle's check (tests/_libs.py).  Seed 1 is the real input; seed 2 is the
-"poison", the same op's valid inputs for another seed, so a read that is not ordered behind the copy of the real
-inputs computes wrong values but never addresses out of bounds.
+CASES is the coverage record: one row per entry point of include/grayskull_b200*.h that takes a gs_b200_stream, with
+a tiled and a generic geometry where the host code has both.  A compute row takes its buffers, its call, its expected
+outputs and its inputs for a seed from tests/_calls.py; the transfer rows describe themselves here.  Seed 1 is the
+real input; seed 2 is the "poison", the same op's valid inputs for another seed, so a read that is not ordered behind
+the copy of the real inputs computes wrong values but never addresses out of bounds.
 
   * CPU: CASES names every such entry point the header declares; the census of blocking or legacy-stream runtime
     calls each object of the library imports, each with its reason.
@@ -15,9 +15,11 @@ inputs computes wrong values but never addresses out of bounds.
     second sleeping stream may have finished, and the clones must be bit-exact.
   * GPU B: every row on two streams at once, at two geometries.
   * GPU C: cudaStreamPerThread from two host threads, ops whose scratch holds values.
-  * GPU D: every row captured into a CUDA graph and replayed with new inputs and changed host parameters.
+  * GPU D: every row captured into a CUDA graph and replayed with new inputs and changed host parameters; a capture
+    that would grow the workspace is refused.
 """
 import ctypes as C
+import glob
 import os
 import re
 import shutil
@@ -28,18 +30,21 @@ import time
 import numpy as np
 import pytest
 
+import _calls as calls
 import _libs as L
 from _gpu import O, frames, lib  # noqa: F401
 
 ROOT = L.ROOT
-FILL = 0xA5                          # what the outputs hold before a call
+POISON = calls.POISON                # what the outputs hold before a call
 SLEEP_MIN_CYCLES = 40_000_000        # ~20 ms at 1.98 GHz
 SLEEP_MAX_CYCLES = 400_000_000       # ~200 ms: the bound on any one sleep
 CAPTURE_UNSUPPORTED = 900            # cudaErrorStreamCaptureUnsupported
 
 
-def _bump(p):
-    """the second geometry of a row (part B): one more frame, two more rows"""
+def _second(p):
+    """the second geometry of a row (part B): the row's own, else one more frame and two more rows"""
+    if "second" in p:
+        return p["second"]
     q = dict(p)
     if "n" in q:
         q["n"] += 1
@@ -53,6 +58,7 @@ def case(cid, fn, **p):
     return cid, fn, p
 
 
+K7X5 = (np.random.default_rng(75).integers(-8, 9, (5, 7)).astype(np.int8).view(np.uint8), 9)
 CASES = [
     case("blur-tma", "gs_b200_blur_batch", w=272, h=70, n=3, r=3),
     case("blur-ragged", "gs_b200_blur_batch", w=100, h=70, n=3, r=9),
@@ -66,11 +72,11 @@ CASES = [
     case("erode-ragged", "gs_b200_erode_batch", w=100, h=37, n=3),
     case("dilate-tma", "gs_b200_dilate_batch", w=272, h=41, n=3),
     case("dilate-ragged", "gs_b200_dilate_batch", w=100, h=37, n=3),
-    case("erode_n-9", "gs_b200_erode_n_batch", w=272, h=70, n=2, it=9),
-    case("erode_n-17", "gs_b200_erode_n_batch", w=272, h=70, n=2, it=17),               # two composed launches
-    case("erode_n-ragged", "gs_b200_erode_n_batch", w=100, h=37, n=3, it=3),            # row / column path
-    case("dilate_n-9", "gs_b200_dilate_n_batch", w=272, h=70, n=2, it=9),
-    case("dilate_n-ragged", "gs_b200_dilate_n_batch", w=100, h=37, n=3, it=4),
+    case("erode_n-9", "gs_b200_erode_n_batch", w=272, h=70, n=2, iters=9),
+    case("erode_n-17", "gs_b200_erode_n_batch", w=272, h=70, n=2, iters=17),               # two composed launches
+    case("erode_n-ragged", "gs_b200_erode_n_batch", w=100, h=37, n=3, iters=3),            # row / column path
+    case("dilate_n-9", "gs_b200_dilate_n_batch", w=272, h=70, n=2, iters=9),
+    case("dilate_n-ragged", "gs_b200_dilate_n_batch", w=100, h=37, n=3, iters=4),
     case("resize-tiled", "gs_b200_resize_batch", w=272, h=60, n=3, dw=200, dh=50),
     case("resize-ragged", "gs_b200_resize_batch", w=100, h=37, n=3, dw=37, dh=50),
     case("downsample-vec", "gs_b200_downsample_batch", w=272, h=41, n=3),
@@ -80,14 +86,14 @@ CASES = [
     case("integral-ragged", "gs_b200_integral_batch", w=100, h=37, n=3),
     case("histogram-vec", "gs_b200_histogram_batch", w=272, h=41, n=3),
     case("histogram-ragged", "gs_b200_histogram_batch", w=100, h=37, n=3),
-    case("otsu-vec", "gs_b200_otsu_threshold_batch", w=272, h=41, n=3),
-    case("otsu-ragged", "gs_b200_otsu_threshold_batch", w=101, h=37, n=3),
+    case("otsu-vec", "gs_b200_otsu_threshold_batch", w=272, h=41, n=3, with_hist=0),
+    case("otsu-ragged", "gs_b200_otsu_threshold_batch", w=101, h=37, n=3, with_hist=0),
     case("threshold-vec", "gs_b200_threshold_batch", w=272, h=41, n=3, t=100),
     case("threshold-ragged", "gs_b200_threshold_batch", w=100, h=37, n=3, t=100),
     case("threshold_each-vec", "gs_b200_threshold_each_batch", w=272, h=41, n=3, offset=10),
     case("threshold_each-ragged", "gs_b200_threshold_each_batch", w=100, h=37, n=3, offset=-20),
-    case("filter-3x3", "gs_b200_filter_batch", w=272, h=41, n=3, k="3x3"),
-    case("filter-7x5", "gs_b200_filter_batch", w=272, h=41, n=3, k="7x5"),
+    case("filter-3x3", "gs_b200_filter_batch", w=272, h=41, n=3, k="sharpen"),
+    case("filter-7x5", "gs_b200_filter_batch", w=272, h=41, n=3, k=K7X5),
     case("match_template-packed", "gs_b200_match_template_batch", w=256, h=60, n=3, tw=30, th=24),
     case("match_template-ragged", "gs_b200_match_template_batch", w=101, h=37, n=3, tw=9, th=4),
     case("find_best_match", "gs_b200_find_best_match_batch", w=101, h=37, n=3),
@@ -95,13 +101,24 @@ CASES = [
     case("blob_corners", "gs_b200_blob_corners", w=100, h=37),
     case("perspective-host", "gs_b200_perspective_correct_batch", w=200, h=150, n=3, dw=90, dh=71, per_frame=0),
     case("perspective-per_frame", "gs_b200_perspective_correct_batch", w=200, h=150, n=3, dw=90, dh=71, per_frame=1),
-    case("fast-tiled", "gs_b200_fast_batch", w=272, h=60, n=3, t=20),
-    case("fast-ragged", "gs_b200_fast_batch", w=101, h=37, n=3, t=10),
-    case("orb-tiled", "gs_b200_orb_extract_batch", w=272, h=60, n=3, t=20),
-    case("orb-ragged", "gs_b200_orb_extract_batch", w=202, h=60, n=3, t=20),
-    case("match_orb", "gs_b200_match_orb_batch", n=3),
-    case("lbp-chunked", "gs_b200_lbp_detect_batch", w=136, h=130, n=3, chunk="1"),
-    case("lbp-ragged", "gs_b200_lbp_detect_batch", w=130, h=130, n=2),
+    case("fast-tiled", "gs_b200_fast_batch", w=272, h=60, n=3, t=20, nkps=400),
+    case("fast-ragged", "gs_b200_fast_batch", w=101, h=37, n=3, t=10, nkps=400),
+    case("orb-tiled", "gs_b200_orb_extract_batch", w=272, h=60, n=3, t=20, nkps=400),
+    case("orb-ragged", "gs_b200_orb_extract_batch", w=202, h=60, n=3, t=20, nkps=400),
+    case("match_orb", "gs_b200_match_orb_batch", n=3, s1=130, s2=90, mm=150),
+    case("lbp-chunked", "gs_b200_lbp_detect_batch", w=136, h=130, n=3, mr=1000, chunk="1"),
+    case("lbp-ragged", "gs_b200_lbp_detect_batch", w=130, h=130, n=2, mr=1000),
+    # the copy kernel (nearest, an unscaled region) or the gather kernel, then the same on a ragged second geometry
+    case("crop_resize-nearest", "gs_b200_crop_resize_batch", w=272, h=70, n=3, dw=64, dh=48, roi=(9, 4, 64, 48), mode=0,
+         second=dict(w=101, h=37, n=2, dw=33, dh=20, roi=(9, 4, 33, 20), mode=0)),
+    case("crop_resize-bilinear", "gs_b200_crop_resize_batch", w=272, h=70, n=3, dw=64, dh=48, roi=(9, 4, 80, 33), mode=1,
+         second=dict(w=101, h=37, n=2, dw=33, dh=20, roi=(9, 4, 80, 33), mode=1)),
+    case("rois_resize-nearest", "gs_b200_rois_resize_batch", w=272, h=70, n=3, dw=64, dh=48, mr=5, mode=0,
+         second=dict(w=101, h=37, n=2, dw=33, dh=20, mr=5, mode=0)),
+    case("rois_resize-bilinear", "gs_b200_rois_resize_batch", w=272, h=70, n=3, dw=64, dh=48, mr=5, mode=1,
+         second=dict(w=101, h=37, n=2, dw=33, dh=20, mr=5, mode=1)),
+    case("orb_pyramid", "gs_b200_orb_pyramid_batch", w=320, h=240, n=3, nkps=600, levels=3, t=20,
+         second=dict(w=264, h=131, n=2, nkps=301, levels=4, t=20)),
     case("memcpy_h2d", "gs_b200_memcpy_h2d", bytes=100003),
     case("memcpy_d2h", "gs_b200_memcpy_d2h", bytes=100003),
     case("memset", "gs_b200_memset", bytes=100003),
@@ -122,13 +139,14 @@ PER_THREAD = ("otsu-ragged", "filter-7x5", "match_template-packed", "find_best_m
 
 # ---- CPU -----------------------------------------------------------------------------------------------------------
 def test_cases_cover_every_stream_entry_point():
-    with open(os.path.join(ROOT, "include", "grayskull_b200.h")) as f:
-        text = re.sub(r"/\*.*?\*/", "", f.read(), flags=re.S)
     declared = set()
-    for m in re.finditer(r"\b(gs_b200_\w+)\s*\(([^)]*)\)\s*;", text):
-        if "gs_b200_stream" in m.group(2):
-            declared.add(m.group(1))
-    assert len(declared) >= 29, sorted(declared)
+    for path in glob.glob(os.path.join(ROOT, "include", "grayskull_b200*.h")):
+        with open(path) as f:
+            text = re.sub(r"/\*.*?\*/", "", f.read(), flags=re.S)
+        for m in re.finditer(r"\b(gs_b200_\w+)\s*\(([^)]*)\)\s*;", text):
+            if "gs_b200_stream" in m.group(2):
+                declared.add(m.group(1))
+    assert len(declared) >= 32, sorted(declared)
     named = {fn for _, fn, _ in CASES}
     assert declared == named, "header entry points without a row: %s; rows naming no entry point: %s" % (
         sorted(declared - named), sorted(named - declared))
@@ -190,304 +208,19 @@ def test_blocking_runtime_calls_census():
 
 
 # ---- GPU: the rows -------------------------------------------------------------------------------------------------
-def _fr(w, h, n, seed):
-    """frames; the poison seed reverses their kinds, so no frame of it equals the real one"""
-    return frames(w, h, n, 1) if seed == 1 else np.ascontiguousarray(frames(w, h, n, 100 + seed)[::-1])
-
-
-def _eq(got, want, what):
-    assert np.array_equal(got, want), what
-
-
-class Spec:
-    """ins: input arrays for a seed (gen); outs: (nbytes, fill, on_host); call(in_ptrs, out_ptrs, stream) -> rc;
-    check(ins, results) with results = the outputs' bytes, then those of the inputs listed in `inplace`"""
-
-    def __init__(self, gen, outs, call, check, host_ins=(), inplace=(), mutate=None, env=None):
-        self.gen, self.outs, self.call, self.check = gen, outs, call, check
-        self.host_ins, self.inplace, self.mutate, self.env = set(host_ins), tuple(inplace), mutate, env or {}
-
-
-def out(nbytes, fill=FILL, host=False):
-    return nbytes, fill, host
-
-
-def _spec(fn, p):
+def _transfer(fn, p):
+    """the rows that move or set bytes -> (spec, inputs for a seed); `host` names the buffer in pinned host memory"""
     import grayskull_b200 as g
-    lib, Od = g.lib(), L.oracle()
-    w, h, n = p.get("w"), p.get("h"), p.get("n")
-    ff = lambda seed: [_fr(w, h, n, seed)]                                   # noqa: E731
-
-    def frames_check(want_fn, shape=None):
-        def check(ins, res):
-            got = res[0].reshape(shape or (n, h, w))
-            for i in range(n):
-                _eq(got[i], want_fn(ins[0][i]), i)
-        return check
-
-    if fn in ("gs_b200_blur_batch", "gs_b200_adaptive_threshold_batch"):
-        r, c = p["r"], p.get("c")
-        if c is None:
-            return Spec(ff, [out(n * w * h)], lambda i, o, s: lib.gs_b200_blur_batch(o[0], i[0], w, h, n, r, s),
-                        frames_check(lambda a: L.o_blur(Od, a, r)))
-        return Spec(ff, [out(n * w * h)],
-                    lambda i, o, s: lib.gs_b200_adaptive_threshold_batch(o[0], i[0], w, h, n, r, c, s),
-                    frames_check(lambda a: L.o_adaptive(Od, a, r, c)))
-    if fn == "gs_b200_sobel_batch":
-        return Spec(ff, [out(n * w * h)], lambda i, o, s: lib.gs_b200_sobel_batch(o[0], i[0], w, h, n, s),
-                    frames_check(lambda a: L.o_sobel(Od, a, FILL)))
-    if fn == "gs_b200_blur_sobel_batch":
-        r = p["r"]
-        return Spec(ff, [out(n * w * h)], lambda i, o, s: lib.gs_b200_blur_sobel_batch(o[0], i[0], w, h, n, r, s),
-                    frames_check(lambda a: L.o_sobel(Od, L.o_blur(Od, a, r), FILL)))
-    if fn in ("gs_b200_erode_batch", "gs_b200_dilate_batch", "gs_b200_erode_n_batch", "gs_b200_dilate_n_batch"):
-        dil, it = "dilate" in fn, p.get("it")
-        f = getattr(lib, fn)
-
-        def want(a):
-            for _ in range(it or 1):
-                a = L.o_morph(Od, a, dil)
-            return a
-        if it is None:
-            return Spec(ff, [out(n * w * h)], lambda i, o, s: f(o[0], i[0], w, h, n, s), frames_check(want))
-        return Spec(ff, [out(n * w * h)], lambda i, o, s: f(o[0], i[0], w, h, n, it, s), frames_check(want))
-    if fn == "gs_b200_resize_batch":
-        dw, dh = p["dw"], p["dh"]
-        return Spec(ff, [out(n * dw * dh)], lambda i, o, s: lib.gs_b200_resize_batch(o[0], dw, dh, i[0], w, h, n, s),
-                    frames_check(lambda a: L.o_resize(Od, a, dw, dh), (n, dh, dw)))
-    if fn == "gs_b200_downsample_batch":
-        return Spec(ff, [out(n * (w // 2) * (h // 2))],
-                    lambda i, o, s: lib.gs_b200_downsample_batch(o[0], i[0], w, h, n, s),
-                    frames_check(lambda a: L.o_down(Od, a), (n, h // 2, w // 2)))
-    if fn == "gs_b200_integral_batch":
-        def check(ins, res):
-            got = res[0].view(np.uint32).reshape(n, h, w)
-            for i in range(n):
-                _eq(got[i], L.o_integral(Od, ins[0][i]), i)
-        return Spec(ff, [out(4 * n * w * h)], lambda i, o, s: lib.gs_b200_integral_batch(o[0], i[0], w, h, n, s),
-                    check, env={"GS_B200_INTEGRAL": p["env"]} if "env" in p else None)
-    if fn == "gs_b200_histogram_batch":
-        def check(ins, res):
-            got = res[0].view(np.uint32).reshape(n, 256)
-            for i in range(n):
-                _eq(got[i], np.bincount(ins[0][i].ravel(), minlength=256), i)
-        return Spec(ff, [out(4 * 256 * n)], lambda i, o, s: lib.gs_b200_histogram_batch(o[0], i[0], w, h, n, s), check)
-    if fn == "gs_b200_otsu_threshold_batch":
-        def check(ins, res):
-            for i in range(n):
-                assert res[0][i] == Od.gso_otsu_threshold(L.ptr(ins[0][i]), w, h), i
-        return Spec(ff, [out(n)], lambda i, o, s: lib.gs_b200_otsu_threshold_batch(o[0], None, i[0], w, h, n, s), check)
-    if fn in ("gs_b200_threshold_batch", "gs_b200_threshold_each_batch"):
-        each = fn.endswith("each_batch")
-
-        def gen(seed):
-            t = np.random.default_rng(seed).integers(0, 256, n).astype(np.uint8)
-            return [_fr(w, h, n, seed)] + ([t] if each else [])
-
-        def check(ins, res):
-            got = res[0].reshape(n, h, w)
-            for i in range(n):
-                want = ins[0][i].copy()
-                Od.gso_threshold(L.ptr(want), w, h, (int(ins[1][i]) + p["offset"]) & 255 if each else p["t"])
-                _eq(got[i], want, i)
-        if each:
-            call = lambda i, o, s: lib.gs_b200_threshold_each_batch(i[0], w, h, n, i[1], p["offset"], s)  # noqa: E731
-        else:
-            call = lambda i, o, s: lib.gs_b200_threshold_batch(i[0], w, h, n, p["t"], s)                  # noqa: E731
-        return Spec(gen, [], call, check, inplace=(0,))
-    if fn == "gs_b200_filter_batch":
-        if p["k"] == "3x3":
-            k, norm = L.filter_kernel("sharpen")
-        else:
-            k = np.random.default_rng(75).integers(-8, 9, (5, 7)).astype(np.int8).view(np.uint8)
-            norm = 9
-        ks, k0 = np.ascontiguousarray(k), np.ascontiguousarray(k).copy()   # ks: the host weights a call reads
-
-        def check(ins, res):
-            got = res[0].reshape(n, h, w)
-            for i in range(n):
-                want = np.zeros((h, w), np.uint8)
-                Od.gso_filter(L.ptr(want), L.ptr(ins[0][i]), w, h, L.ptr(k0), k0.shape[1], k0.shape[0], norm)
-                _eq(got[i], want, i)
-
-        def mutate():
-            ks[:] = 1
-        return Spec(ff, [out(n * w * h)],
-                    lambda i, o, s: lib.gs_b200_filter_batch(o[0], i[0], w, h, n, ks.ctypes.data, ks.shape[1], ks.shape[0],
-                                                             norm, s), check, mutate=mutate)
-    if fn == "gs_b200_match_template_batch":
-        tw, th = p["tw"], p["th"]
-        rw, rh = w - tw + 1, h - th + 1
-
-        def gen(seed):
-            fr = _fr(w, h, n, seed)
-            return [fr, np.ascontiguousarray(fr[1, 5 + seed:5 + seed + th, 10 + seed:10 + seed + tw])]
-
-        def check(ins, res):
-            got = res[0].reshape(n, rh, rw)
-            for i in range(n):
-                want = np.zeros((rh, rw), np.uint8)
-                Od.gso_match_template(L.ptr(ins[0][i]), w, h, L.ptr(ins[1]), tw, th, L.ptr(want))
-                _eq(got[i], want, i)
-        return Spec(gen, [out(n * rw * rh)],
-                    lambda i, o, s: lib.gs_b200_match_template_batch(o[0], i[0], w, h, n, i[1], tw, th, s), check)
-    if fn == "gs_b200_find_best_match_batch":
-        px = w * h
-
-        def gen(seed):
-            rng = np.random.default_rng(px + seed)
-            return [(rng.integers(0, 250, (n, px)) * (rng.random((n, px)) < 0.5)).astype(np.uint8)]
-
-        def check(ins, res):
-            got = res[0].view(np.uint32).reshape(n, 2)
-            for i in range(n):
-                b = Od.gso_find_best_match(L.ptr(np.ascontiguousarray(ins[0][i])), w, h)
-                assert tuple(got[i]) == (b % w, b // w), i
-        return Spec(gen, [out(8 * n)], lambda i, o, s: lib.gs_b200_find_best_match_batch(o[0], i[0], w, h, n, s), check)
-    if fn == "gs_b200_blobs_batch":
-        nb = p["nb"]
-
-        def check(ins, res):
-            labels = res[0].view(np.uint16).reshape(n, h, w)
-            blobs, counts = res[1].view(L.BLOB_DTYPE).reshape(n, nb), res[2].view(np.uint32)
-            for i in range(n):
-                wl, wb = _o_blobs(Od, ins[0][i], nb)
-                assert counts[i] == len(wb) and np.array_equal(labels[i], wl), i
-                assert L.blob_fields(blobs[i, :counts[i]]) == L.blob_fields(wb), i
-        return Spec(lambda seed: [np.stack([L.binary_like(w, h, 50 * seed + i) for i in range(n)])],
-                    [out(2 * n * w * h), out(32 * n * nb), out(4 * n)],
-                    lambda i, o, s: lib.gs_b200_blobs_batch(i[0], w, h, n, o[0], o[1], o[2], nb, s), check)
-    if fn == "gs_b200_blob_corners":
-        def gen(seed):
-            a = L.binary_like(w, h, 7 + seed)
-            labels, blobs = _o_blobs(Od, a, 300)
-            j = int(np.argmax(blobs["area"]))
-            return [a, labels, np.ascontiguousarray(blobs[j:j + 1])]
-
-        def check(ins, res):
-            want = np.zeros((4, 2), np.uint32)
-            Od.gso_blob_corners(L.ptr(ins[0]), w, h, L.ptr(ins[1]), L.ptr(ins[2]), L.ptr(want))
-            _eq(res[0].view(np.uint32).reshape(4, 2), want, "corners")
-        return Spec(gen, [out(32)], lambda i, o, s: lib.gs_b200_blob_corners(i[0], w, h, i[1], i[2], o[0], s), check)
-    if fn == "gs_b200_perspective_correct_batch":
-        dw, dh = p["dw"], p["dh"]
-        q_host = np.random.default_rng(5).integers(0, 140, (4, 2)).astype(np.uint32)
-        q0 = q_host.copy()
-
-        def gen(seed):
-            fr = _fr(w, h, n, seed)
-            return [fr, np.random.default_rng(5 + seed).integers(0, 140, (n, 4, 2)).astype(np.uint32)] if p["per_frame"] \
-                else [fr]
-
-        def check(ins, res):
-            got = res[0].reshape(n, dh, dw)
-            for i in range(n):
-                want = np.empty((dh, dw), np.uint8)
-                q = np.ascontiguousarray(ins[1][i]) if p["per_frame"] else q0
-                Od.gso_perspective_correct(L.ptr(want), dw, dh, L.ptr(ins[0][i]), w, h, L.ptr(q))
-                _eq(got[i], want, i)
-
-        def mutate():
-            q_host[:] = 0
-        if p["per_frame"]:
-            call = lambda i, o, s: lib.gs_b200_perspective_correct_batch(o[0], dw, dh, i[0], w, h, n, i[1], 1, s)  # noqa
-        else:
-            call = lambda i, o, s: lib.gs_b200_perspective_correct_batch(o[0], dw, dh, i[0], w, h, n,  # noqa: E731
-                                                                         q_host.ctypes.data, 0, s)
-        return Spec(gen, [out(n * dw * dh)], call, check, mutate=None if p["per_frame"] else mutate)
-    if fn in ("gs_b200_fast_batch", "gs_b200_orb_extract_batch"):
-        orb, t, nk = "orb" in fn, p["t"], 400
-        sm_fill = 0 if orb else FILL
-
-        def gen(seed):
-            fr = _fr(w, h, n, seed)
-            fr[seed % n] = L.natural_like(w, h, 90 + seed)            # corners in every batch
-            return [fr]
-
-        def check(ins, res):
-            sm = res[0].reshape(n, h, w)
-            kps, counts = res[1].view(np.uint32).reshape(n, nk, 12), res[2].view(np.uint32)
-            for i in range(n):
-                so = np.full((h, w), sm_fill, np.uint8)
-                want = L.o_orb(Od, ins[0][i], so, nk, t) if orb else L.o_fast(Od, ins[0][i], so, nk, t)
-                got = np.ascontiguousarray(kps[i, :counts[i]]).view(L.KP_DTYPE).reshape(-1)
-                assert got.tobytes() == want.tobytes(), (i, len(got), len(want))
-                if not orb:
-                    _eq(sm[i], so, i)
-            assert counts.sum() > 0
-        f = getattr(lib, fn)
-        return Spec(gen, [out(n * w * h, sm_fill), out(48 * n * nk), out(4 * n)],
-                    lambda i, o, s: f(i[0], w, h, n, o[0], o[1], o[2], nk, t, s), check)
-    if fn == "gs_b200_match_orb_batch":
-        s1, s2, mm = 130, 90, 150
-        md = {"max_distance": 60.0}
-        sizes = ((120, 90), (7, 0), (130, 61), (40, 75))
-
-        def gen(seed):
-            rng = np.random.default_rng(16 + seed)
-            sets = [L.desc_sets(rng, *sizes[(i + seed) % 4]) for i in range(n)]
-            k1, k2 = np.zeros((n, s1), L.KP_DTYPE), np.zeros((n, s2), L.KP_DTYPE)
-            for i, (a, b) in enumerate(sets):
-                k1[i, :len(a)], k2[i, :len(b)] = a, b
-            return [k1, k2, np.array([len(a) for a, _ in sets], np.uint32), np.array([len(b) for _, b in sets], np.uint32)]
-
-        def check(ins, res):
-            counts, m = res[1].view(np.uint32), res[0].view(np.uint32).reshape(n, mm, 3)
-            for i in range(n):
-                want = L.o_match(Od, ins[0][i, :ins[2][i]], ins[1][i, :ins[3][i]], mm, 60.0)
-                assert counts[i] == len(want) and np.ascontiguousarray(m[i, :counts[i]]).tobytes() == want.tobytes(), i
-
-        def mutate():
-            md["max_distance"] = 1.0
-        return Spec(gen, [out(12 * n * mm), out(4 * n)],
-                    lambda i, o, s: lib.gs_b200_match_orb_batch(i[0], i[2], s1, i[1], i[3], s2, n, o[0], o[1], mm,
-                                                                md["max_distance"], s), check, mutate=mutate)
-    if fn == "gs_b200_lbp_detect_batch":
-        from grayskull_b200._lib import load_cascade
-        cas, cas0, mr = load_cascade(), L.HostCascade(), 1000
-        lena = np.load(os.path.join(ROOT, "tests", "golden", "lena_golden.npz"))["lena"]      # 128 x 128, faces found
-
-        def gen(seed):
-            fr = [np.pad(np.roll(lena, 4 * (i + seed), axis=1), ((0, h - 128), (0, w - 128)), mode="edge")
-                  if (i + seed) % 2 else L.natural_like(w, h, 40 + i + 10 * seed) for i in range(n)]
-            return [np.stack([L.o_integral(Od, f) for f in fr])]
-
-        def check(ins, res):
-            counts, rects = res[1].view(np.uint32), res[0].view(np.uint32).reshape(n, mr, 4)
-            for i in range(n):
-                want = L.o_detect(Od, cas0, ins[0][i], mr, 1.1, 1.0, 4.0, 2)
-                assert np.ascontiguousarray(rects[i, :counts[i]]).tobytes() == want.tobytes(), (i, counts[i], len(want))
-            assert counts.sum() > 0
-
-        def mutate():
-            cas.arrays["stage_threshold"][:] = 1e9
-        return Spec(gen, [out(16 * n * mr), out(4 * n)],
-                    lambda i, o, s: lib.gs_b200_lbp_detect_batch(cas.ptr, i[0], w, h, n, o[0], o[1], mr, 1.1, 1.0, 4.0,
-                                                                 2, s), check, mutate=mutate,
-                    env={"GS_B200_LBP_CHUNK_FRAMES": p["chunk"]} if "chunk" in p else None)
-    if fn in ("gs_b200_memcpy_h2d", "gs_b200_memcpy_d2h", "gs_b200_memset"):
-        nbytes = p["bytes"]
-        gen = lambda seed: [np.random.default_rng(seed).integers(0, 256, nbytes).astype(np.uint8)]  # noqa: E731
-        if fn == "gs_b200_memset":
-            return Spec(lambda seed: [], [out(nbytes)], lambda i, o, s: lib.gs_b200_memset(o[0], 0x3C, nbytes, s),
-                        lambda ins, res: _eq(res[0], np.full(nbytes, 0x3C, np.uint8), "memset"))
-        h2d = fn.endswith("h2d")
-        return Spec(gen, [out(nbytes, host=not h2d)], lambda i, o, s: getattr(lib, fn)(o[0], i[0], nbytes, s),
-                    lambda ins, res: _eq(res[0], ins[0], fn), host_ins=(0,) if h2d else ())
+    lib, nb = g.lib(), p.get("bytes", 0)
     if fn == "gs_b200_stream_sync":
-        return Spec(lambda seed: [], [], lambda i, o, s: lib.gs_b200_stream_sync(s), lambda ins, res: None)
-    raise KeyError(fn)
-
-
-def _o_blobs(Od, a, nb):
-    h, w = a.shape
-    labels, blobs = np.zeros((h, w), np.uint16), np.zeros(nb, L.BLOB_DTYPE)
-    m = Od.gso_blobs(L.ptr(a), w, h, L.ptr(labels), L.ptr(blobs), nb)
-    return labels, blobs[:m]
-
-
-def _bytes(a):
-    return np.frombuffer(np.ascontiguousarray(a).tobytes(), np.uint8)
+        return calls.Spec({}, {}, lambda P, n, s: lib.gs_b200_stream_sync(s), lambda ins, bf: {}), lambda seed: {}
+    if fn == "gs_b200_memset":
+        return calls.Spec({}, {"dst": nb}, lambda P, n, s: lib.gs_b200_memset(P["dst"], 0x3C, nb, s),
+                          lambda ins, bf: {"dst": np.full(nb, 0x3C, np.uint8)}), lambda seed: {}
+    sp = calls.Spec({"src": nb}, {"dst": nb}, lambda P, n, s: getattr(lib, fn)(P["dst"], P["src"], nb, s),
+                    lambda ins, bf: {"dst": ins["src"]})
+    sp.host = {"src"} if fn.endswith("h2d") else {"dst"}
+    return sp, lambda seed: {"src": np.random.default_rng(seed).integers(0, 256, (1, nb)).astype(np.uint8)}
 
 
 class Run:
@@ -496,57 +229,54 @@ class Run:
 
     def __init__(self, fn, p):
         import torch
-        self.fn, self.p, self.spec = fn, p, _spec(fn, p)
-        self.data = {seed: self.spec.gen(seed) for seed in (1, 2)}
-        self.src = {seed: [torch.from_numpy(_bytes(a).copy()).cuda() for a in arrs] for seed, arrs in self.data.items()}
-        self.ins = []
-        for k, a in enumerate(self.src[2]):
-            t = torch.empty(a.numel(), dtype=torch.uint8, pin_memory=True) if k in self.spec.host_ins else torch.empty_like(a)
-            t.copy_(a)
-            self.ins.append(t)
-        self.outs = [torch.empty(nb, dtype=torch.uint8, pin_memory=True) if host else
-                     torch.empty(nb, dtype=torch.uint8, device="cuda") for nb, _, host in self.spec.outs]
+        self.fn, self.n = fn, p.get("n", 1)
+        if fn.endswith(("_batch", "blob_corners")):
+            self.spec, gen = calls.spec(fn, p), lambda seed: calls.inputs(fn, p, self.n, seed)
+        else:
+            self.spec, gen = _transfer(fn, p)
+        host = getattr(self.spec, "host", ())
+        self.data = {seed: gen(seed) for seed in (1, 2)}
+        self.src = {seed: {b: torch.from_numpy(calls.flat(x, 1 if b in self.spec.shared else self.n)).cuda()
+                           for b, x in d.items()} for seed, d in self.data.items()}
+        self.ins = {b: torch.empty(a.numel(), dtype=torch.uint8, pin_memory=True) if b in host else torch.empty_like(a)
+                    for b, a in self.src[2].items()}
+        for b, t in self.ins.items():
+            t.copy_(self.src[2][b])
+        self.before = calls.filled(self.spec, self.n)
+        self.outs = {b: torch.empty(calls.flat(x, self.n).size, dtype=torch.uint8, pin_memory=b in host,
+                                    device="cpu" if b in host else "cuda") for b, x in self.before.items()}
         torch.cuda.synchronize()
 
     def call(self, s):
         """the library call on torch stream s (None: cudaStreamPerThread) -> rc"""
         handle = C.c_void_p(2) if s is None else C.c_void_p(s.cuda_stream)
-        old = {k: os.environ.get(k) for k in self.spec.env}
-        os.environ.update(self.spec.env)
-        try:
-            return self.spec.call([t.data_ptr() for t in self.ins], [t.data_ptr() for t in self.outs], handle)
-        finally:
-            for k, v in old.items():
-                if v is None:
-                    os.environ.pop(k, None)
-                else:
-                    os.environ[k] = v
+        return self.spec.call({b: t.data_ptr() for b, t in dict(self.ins, **self.outs).items()}, self.n, handle)
 
     def stage(self, s, seed):
-        """enqueue on s: the inputs of `seed` over the device inputs, the fill over the device outputs (host outputs
+        """enqueue on s: the inputs of `seed` over the device inputs, the poison over the device outputs (host outputs
         are filled now, on the host)"""
         import torch
         with torch.cuda.stream(s):
-            for t, a in zip(self.ins, self.src[seed]):
-                t.copy_(a, non_blocking=True)
-            for t, (_, fill, host) in zip(self.outs, self.spec.outs):
-                t.fill_(fill)
+            for b, t in self.ins.items():
+                t.copy_(self.src[seed][b], non_blocking=True)
+            for t in self.outs.values():
+                t.fill_(POISON)
 
     def results(self):
-        return self.outs + [self.ins[k] for k in self.spec.inplace]
+        return {b: self.outs[b] if b in self.outs else self.ins[b] for b in self.spec.outs}
 
     def grab(self, s):
         """enqueue on s: clones of the device results (host results are read after the sync)"""
         import torch
         with torch.cuda.stream(s):
-            return [t if not t.is_cuda else t.clone() for t in self.results()]
+            return {b: t.clone() if t.is_cuda else t for b, t in self.results().items()}
 
     def verify(self, got, seed, what=""):
-        res = [g.cpu().numpy() for g in got]
-        try:
-            self.spec.check(self.data[seed], res)
-        except AssertionError as e:
-            raise AssertionError("%s%s (inputs of seed %d): %s" % (self.fn, what, seed, e)) from None
+        want = self.spec.expect(self.data[seed], self.before)
+        for b, t in got.items():
+            g, w = t.cpu().numpy(), calls.flat(want[b], self.n)
+            assert np.array_equal(g, w), "%s%s (inputs of seed %d): %s: byte %d of %d differs" % (
+                self.fn, what, seed, b, int(np.argmax(g != w)), g.size)
 
     def run_sync(self, s, seed=2):
         """one plain call on s, checked: the warm-up (sizes the workspace, builds the LBP plan, the ORB tables)"""
@@ -627,13 +357,13 @@ def test_single_image_calls_follow_the_legacy_stream(lib):
     from grayskull_b200._lib import Image
     Od = L.oracle()
     w, h = 272, 70
-    a = _fr(w, h, 1, 1)[0]
+    a = frames(w, h, 1, 1)[0]
     src = torch.zeros((h, w), dtype=torch.uint8, device="cuda")
     dst = torch.zeros_like(src)
     real = torch.from_numpy(a).cuda()
     torch.cuda.synchronize()
     for op in ("blur", "sobel"):
-        dst.fill_(FILL)
+        dst.fill_(POISON)
         src.zero_()
         torch.cuda.synchronize()
         stream = torch.cuda.default_stream()
@@ -645,8 +375,8 @@ def test_single_image_calls_follow_the_legacy_stream(lib):
             want = L.o_blur(Od, a, 3)
         else:
             lib.gs_sobel(di, si)
-            want = L.o_sobel(Od, a, FILL)
-        _eq(dst.cpu().numpy(), want, op)
+            want = L.o_sobel(Od, a, POISON)
+        assert np.array_equal(dst.cpu().numpy(), want), op
 
 
 # ---- GPU B: two streams at once ------------------------------------------------------------------------------------
@@ -655,7 +385,7 @@ def test_single_image_calls_follow_the_legacy_stream(lib):
 def test_two_streams_at_once(lib, head_sleep):
     import torch
     s0, s1 = torch.cuda.Stream(), torch.cuda.Stream()
-    pairs = [(Run(fn, p), Run(fn, _bump(p))) for cid, fn, p in CASES if cid not in WAITS]
+    pairs = [(Run(fn, p), Run(fn, _second(p))) for cid, fn, p in CASES if cid not in WAITS]
     for r0, r1 in pairs:                         # each stream's workspace sized for its own geometry
         r0.run_sync(s0)
         r1.run_sync(s1)
@@ -697,7 +427,7 @@ def test_stream_per_thread_has_per_thread_scratch(lib):
     rows = {cid: (fn, p) for cid, fn, p in CASES}
     runs = {who: [Run(*rows[cid]) for cid in PER_THREAD] for who in "AB"}
     long_call, long_dst, long_want = _long_filter()
-    staged = [[_bytes(a) for a in r.data[1]] for r in runs["B"]]
+    staged = [{b: t.cpu().numpy() for b, t in r.src[1].items()} for r in runs["B"]]
     torch.cuda.synchronize()
     a_returned, errors, got = threading.Event(), [], {}
 
@@ -725,13 +455,13 @@ def test_stream_per_thread_has_per_thread_scratch(lib):
             a_returned.wait(60)
             # nothing on the legacy stream from here on: it would wait for thread A's stream
             for r, host in zip(runs["B"], staged):
-                for t, a in zip(r.ins, host):        # the real inputs, on this thread's stream only
-                    _ok(lib.gs_b200_memcpy_h2d(t.data_ptr(), a.ctypes.data, a.nbytes, C.c_void_p(2)), "h2d")
-                for t, (nb, fill, _) in zip(r.outs, r.spec.outs):
-                    _ok(lib.gs_b200_memset(t.data_ptr(), fill, nb, C.c_void_p(2)), "memset")
+                for b, t in r.ins.items():            # the real inputs, on this thread's stream only
+                    _ok(lib.gs_b200_memcpy_h2d(t.data_ptr(), host[b].ctypes.data, host[b].nbytes, C.c_void_p(2)), "h2d")
+                for t in r.outs.values():
+                    _ok(lib.gs_b200_memset(t.data_ptr(), POISON, t.numel(), C.c_void_p(2)), "memset")
                 _ok(r.call(None), r.fn)
             sync()
-            got["B"] = [[t.cpu() for t in r.results()] for r in runs["B"]]
+            got["B"] = [{b: t.cpu() for b, t in r.results().items()} for r in runs["B"]]
         except BaseException as e:   # noqa: B036
             errors.append(e)
 
@@ -786,17 +516,28 @@ def test_graph_capture_and_replay(lib, fn, p, request):
         run.verify(got, seed, " replay")
 
 
+GROW = [pytest.param("gs_b200_otsu_threshold_batch", dict(w=101, h=37, n=2, with_hist=0),
+                     dict(w=101, h=37, n=64, with_hist=0), False, id="otsu"),
+        # torch may report the invalidated capture itself; the call's status is what counts
+        pytest.param("gs_b200_orb_pyramid_batch", dict(w=128, h=96, n=1, nkps=50, levels=3, t=20),
+                     dict(w=512, h=384, n=3, nkps=2000, levels=3, t=20), True, id="orb_pyramid")]
+
+
 @pytest.mark.gpu
-def test_workspace_cannot_grow_inside_a_capture(lib):
+@pytest.mark.parametrize("fn,small,big,torch_may_refuse", GROW)
+def test_workspace_cannot_grow_inside_a_capture(lib, fn, small, big, torch_may_refuse):
     """a capture that would need a larger arena fails with a clear error and leaves the arena as it was"""
     import torch
-    small, big = Run("gs_b200_otsu_threshold_batch", dict(w=101, h=37, n=2)), \
-        Run("gs_b200_otsu_threshold_batch", dict(w=101, h=37, n=64))
+    small, big = Run(fn, small), Run(fn, big)
     s = torch.cuda.Stream()
     small.run_sync(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g, stream=s):
-        rc = big.call(s)
+    g, rc = torch.cuda.CUDAGraph(), None
+    try:
+        with torch.cuda.graph(g, stream=s):
+            rc = big.call(s)
+    except RuntimeError:
+        if not torch_may_refuse:
+            raise
     assert rc == CAPTURE_UNSUPPORTED, (rc, lib.gs_b200_last_error())
     assert b"capturing" in lib.gs_b200_last_error()
     small.run_sync(s, 1)                         # the old arena still serves the small geometry
