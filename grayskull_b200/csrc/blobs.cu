@@ -373,40 +373,44 @@ struct Quad {
 __global__ void __launch_bounds__(256)
 k_perspective(uint8_t *__restrict__ dst, unsigned dw, unsigned dh, const uint8_t *__restrict__ src, unsigned sw, unsigned sh,
               unsigned n, const unsigned *__restrict__ corners /* n x 8 (device) or null */, Quad q0) {
-  const unsigned x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  const unsigned x = blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= dw) return;
   const float wm = __fsub_rn((float)dw, 1.0f), hm = __fsub_rn((float)dh, 1.0f);
   const float mx = __fsub_rn((float)sw, 1.0f), my = __fsub_rn((float)sh, 1.0f);
-  const float u = __fdiv_rn((float)x, wm), v = __fdiv_rn((float)y, hm);
-  const float omu = __fsub_rn(1.0f, u), omv = __fsub_rn(1.0f, v);
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    Quad q = q0;
-    if (corners) {
+  const float u = __fdiv_rn((float)x, wm);
+  const float omu = __fsub_rn(1.0f, u);
+  for (unsigned y = blockIdx.y; y < dh; y += gridDim.y) {   // grid y: <= 65535 rows
+    const float v = __fdiv_rn((float)y, hm);
+    const float omv = __fsub_rn(1.0f, v);
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      Quad q = q0;
+      if (corners) {
 #pragma unroll
-      for (int i = 0; i < 4; i++) q.x[i] = (float)corners[f * 8 + 2 * i], q.y[i] = (float)corners[f * 8 + 2 * i + 1];
+        for (int i = 0; i < 4; i++) q.x[i] = (float)corners[f * 8 + 2 * i], q.y[i] = (float)corners[f * 8 + 2 * i + 1];
+      }
+      const float top_x = __fadd_rn(__fmul_rn(q.x[0], omu), __fmul_rn(q.x[1], u));
+      const float top_y = __fadd_rn(__fmul_rn(q.y[0], omu), __fmul_rn(q.y[1], u));
+      const float bot_x = __fadd_rn(__fmul_rn(q.x[3], omu), __fmul_rn(q.x[2], u));
+      const float bot_y = __fadd_rn(__fmul_rn(q.y[3], omu), __fmul_rn(q.y[2], u));
+      float sx = __fadd_rn(__fmul_rn(top_x, omv), __fmul_rn(bot_x, v));
+      float sy = __fadd_rn(__fmul_rn(top_y, omv), __fmul_rn(bot_y, v));
+      sx = sx < mx ? sx : mx;                             // GS_MIN(src_x, w - 1): a NaN falls to w - 1
+      sy = sy < my ? sy : my;
+      sx = 0.0f > sx ? 0.0f : sx;                         // GS_MAX(0, .)
+      sy = 0.0f > sy ? 0.0f : sy;
+      const unsigned x0 = (unsigned)sx, y0 = (unsigned)sy;
+      const unsigned x1 = min(x0 + 1, sw - 1), y1 = min(y0 + 1, sh - 1);
+      const float dx = __fsub_rn(sx, (float)x0), dy = __fsub_rn(sy, (float)y0);
+      const uint8_t *s = src + (size_t)f * sw * sh;
+      const float c00 = (float)s[(size_t)y0 * sw + x0], c01 = (float)s[(size_t)y0 * sw + x1];
+      const float c10 = (float)s[(size_t)y1 * sw + x0], c11 = (float)s[(size_t)y1 * sw + x1];
+      const float omx = __fsub_rn(1.0f, dx), omy = __fsub_rn(1.0f, dy);
+      float acc = __fmul_rn(__fmul_rn(c00, omx), omy);
+      acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(c01, dx), omy));
+      acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(c10, omx), dy));
+      acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(c11, dx), dy));
+      dst[(size_t)f * dw * dh + (size_t)y * dw + x] = (uint8_t)(unsigned)acc;
     }
-    const float top_x = __fadd_rn(__fmul_rn(q.x[0], omu), __fmul_rn(q.x[1], u));
-    const float top_y = __fadd_rn(__fmul_rn(q.y[0], omu), __fmul_rn(q.y[1], u));
-    const float bot_x = __fadd_rn(__fmul_rn(q.x[3], omu), __fmul_rn(q.x[2], u));
-    const float bot_y = __fadd_rn(__fmul_rn(q.y[3], omu), __fmul_rn(q.y[2], u));
-    float sx = __fadd_rn(__fmul_rn(top_x, omv), __fmul_rn(bot_x, v));
-    float sy = __fadd_rn(__fmul_rn(top_y, omv), __fmul_rn(bot_y, v));
-    sx = sx < mx ? sx : mx;                             // GS_MIN(src_x, w - 1): a NaN falls to w - 1
-    sy = sy < my ? sy : my;
-    sx = 0.0f > sx ? 0.0f : sx;                         // GS_MAX(0, .)
-    sy = 0.0f > sy ? 0.0f : sy;
-    const unsigned x0 = (unsigned)sx, y0 = (unsigned)sy;
-    const unsigned x1 = min(x0 + 1, sw - 1), y1 = min(y0 + 1, sh - 1);
-    const float dx = __fsub_rn(sx, (float)x0), dy = __fsub_rn(sy, (float)y0);
-    const uint8_t *s = src + (size_t)f * sw * sh;
-    const float c00 = (float)s[(size_t)y0 * sw + x0], c01 = (float)s[(size_t)y0 * sw + x1];
-    const float c10 = (float)s[(size_t)y1 * sw + x0], c11 = (float)s[(size_t)y1 * sw + x1];
-    const float omx = __fsub_rn(1.0f, dx), omy = __fsub_rn(1.0f, dy);
-    float acc = __fmul_rn(__fmul_rn(c00, omx), omy);
-    acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(c01, dx), omy));
-    acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(c10, omx), dy));
-    acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(c11, dx), dy));
-    dst[(size_t)f * dw * dh + (size_t)y * dw + x] = (uint8_t)(unsigned)acc;
   }
 }
 
@@ -461,13 +465,12 @@ int gs_b200_perspective_correct_batch(uint8_t *dst, unsigned dw, unsigned dh, co
                                       unsigned n, const struct gs_point *corners, int per_frame, gs_b200_stream s) {
   GSB_ASSERT(dst && dw > 0 && dh > 0 && src && sw > 0 && sh > 0 && corners);   // reference :424
   if (n == 0) return 0;
-  GSB_ASSERT(dh <= 65535u);
   gsb::Quad q = {};
   const unsigned *dev = nullptr;
   if (per_frame) dev = reinterpret_cast<const unsigned *>(corners);             // n x 4 points in DEVICE memory
   else
     for (int i = 0; i < 4; i++) q.x[i] = (float)corners[i].x, q.y[i] = (float)corners[i].y;   // 4 points in HOST memory
-  dim3 grid((dw + 255) / 256, dh, n < 64u ? n : 64u);
+  dim3 grid((dw + 255) / 256, dh < gsb::GRID_FRAMES ? dh : gsb::GRID_FRAMES, n < 64u ? n : 64u);
   GSB_LAUNCH(gsb::k_perspective, grid, 256, 0, static_cast<cudaStream_t>(s), dst, dw, dh, src, sw, sh, n, dev, q);
   return 0;
 }

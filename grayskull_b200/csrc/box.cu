@@ -173,7 +173,8 @@ __device__ __forceinline__ void unpack_pairs(uint2 v, uint32_t (&p)[4]) {
 
 template <int R, bool ADAPTIVE>
 __global__ void __launch_bounds__(BX_THREADS)
-k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, unsigned w, unsigned h, int cparam) {
+k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, unsigned w, unsigned h, int cparam,
+          unsigned ty0 /* first row tile of the launch: for_row_groups */) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint32_t *tile = reinterpret_cast<uint32_t *>(smem_raw);
   float2 *magic = reinterpret_cast<float2 *>(smem_raw + BX_TILE_WORDS * 4);
@@ -183,7 +184,7 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 
   const unsigned frame = blockIdx.z;
   const int xb = (int)blockIdx.x * BX_STRIDE - 16;   // image column of tile byte 0 (16-B aligned)
-  const int y0 = (int)blockIdx.y * BX_TH;
+  const int y0 = (int)(blockIdx.y + ty0) * BX_TH;
   // every window of this tile's outputs lies inside the image: no clipping, no partial rows/cols
   const bool interior = xb + 8 - R >= 0 && xb + 8 + BX_STRIDE - 1 + R <= (int)w - 1 && y0 - R >= 0 &&
                         y0 + BX_TH - 1 + R <= (int)h - 1;
@@ -369,7 +370,8 @@ __device__ __forceinline__ void st_cs_7of8(uint8_t *p, uint2 v, bool left) {
 
 template <int R>
 __global__ void __launch_bounds__(BS_THREADS, 3)
-k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, unsigned w, unsigned h) {
+k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, unsigned w, unsigned h,
+                 unsigned ty0 /* first row tile of the launch: for_row_groups */) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const uint32_t *in = reinterpret_cast<const uint32_t *>(smem_raw);          // input row i = image row Y - 8 + i
   unsigned char *bl = smem_raw + BS_IN_BYTES;                                 // blurred row i = image row Y + i
@@ -381,7 +383,7 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
 
   const unsigned frame = blockIdx.z;
   const int xb = (int)blockIdx.x * BS_STRIDE - 16;   // image column of tile byte 0 (16-B aligned)
-  const int y0 = (int)blockIdx.y * BS_TH;            // first sobel row of the tile
+  const int y0 = (int)(blockIdx.y + ty0) * BS_TH;    // first sobel row of the tile
   const int Y = y0 - 1;                              // first blurred row
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
@@ -1059,21 +1061,22 @@ template <bool ADAPTIVE>
 __global__ void k_box_generic(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, unsigned w,
                               unsigned h, unsigned n, unsigned r, int cparam) {
   const unsigned x = blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= w || y >= h) return;
+  if (x >= w) return;
   const unsigned xa = x > r ? x - r : 0, xb = min(x + (unsigned long long)r, (unsigned long long)w - 1);
-  const unsigned ya = y > r ? y - r : 0, yb = min(y + (unsigned long long)r, (unsigned long long)h - 1);
-  const unsigned count = (xb - xa + 1) * (yb - ya + 1);
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint8_t *s = src + (size_t)f * w * h;
-    unsigned sum = 0;
-    for (unsigned yy = ya; yy <= yb; yy++)
-      for (unsigned xx = xa; xx <= xb; xx++) sum += s[(size_t)yy * w + xx];
-    const unsigned mean = sum / count;
-    uint8_t v;
-    if (ADAPTIVE) v = ((int)s[(size_t)y * w + x] > (int)(mean - (unsigned)cparam)) ? 255 : 0;
-    else v = (uint8_t)mean;
-    dst[(size_t)f * w * h + (size_t)y * w + x] = v;
+  for (unsigned y = blockIdx.y * blockDim.y + threadIdx.y; y < h; y += gridDim.y * blockDim.y) {   // grid y: <= 65535 row tiles
+    const unsigned ya = y > r ? y - r : 0, yb = min(y + (unsigned long long)r, (unsigned long long)h - 1);
+    const unsigned count = (xb - xa + 1) * (yb - ya + 1);
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint8_t *s = src + (size_t)f * w * h;
+      unsigned sum = 0;
+      for (unsigned yy = ya; yy <= yb; yy++)
+        for (unsigned xx = xa; xx <= xb; xx++) sum += s[(size_t)yy * w + xx];
+      const unsigned mean = sum / count;
+      uint8_t v;
+      if (ADAPTIVE) v = ((int)s[(size_t)y * w + x] > (int)(mean - (unsigned)cparam)) ? 255 : 0;
+      else v = (uint8_t)mean;
+      dst[(size_t)f * w * h + (size_t)y * w + x] = v;
+    }
   }
 }
 
@@ -1098,9 +1101,10 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
         k_box_tma<5, ADAPTIVE>, k_box_tma<6, ADAPTIVE>, k_box_tma<7, ADAPTIVE>};
     // tile t covers output columns [240 t - 8, 240 t + 232)
     const unsigned tiles_x = (w + 8 + BX_STRIDE - 1) / BX_STRIDE, tiles_y = (h + BX_TH - 1) / BX_TH;
-    GSB_ASSERT(tiles_y <= 65535u);   // grid y limit (z is at most one frame group)
-    GSB_LAUNCH(box_tma_fn[r - 1], dim3(tiles_x, tiles_y, n), BX_THREADS, BX_SMEM, s, tmap, dst, w, h, cparam);
-    return 0;
+    return for_row_groups(tiles_y, [&](unsigned t0, unsigned c) {
+      return launch(__FILE__, __LINE__, box_tma_fn[r - 1], dim3(tiles_x, c, n), BX_THREADS, BX_SMEM, s, tmap, dst, w, h,
+                    cparam, t0);
+    });
   }
   if (banded) {
     // radius-independent path: warp-autonomous 256-column segments, u32 window sums (k_box_wide)
@@ -1113,8 +1117,7 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
     if (bands > max_bands) bands = max_bands;
     if (bands < 1) bands = 1;
     int BH = (int)((h + bands - 1) / bands);
-    const unsigned gy = (h + BH - 1) / BH;
-    GSB_ASSERT(gy <= 65535u);
+    const unsigned gy = (h + BH - 1) / BH;   // <= bands <= 24 per SM
     float minv = 0.0f;
     const int fast_ok = (r <= 63 && box_wide_magic((2 * r + 1) * (2 * r + 1), &minv)) ? 1 : 0;
     const bool aligned = w % 8 == 0 && reinterpret_cast<uintptr_t>(src) % 8 == 0 && reinterpret_cast<uintptr_t>(dst) % 8 == 0;
@@ -1144,7 +1147,7 @@ static int launch_box(uint8_t *dst, const uint8_t *src, unsigned w, unsigned h, 
     GSB_LAUNCH(k_box_wide<ADAPTIVE>, grid, 128, 0, s, dst, src, (int)w, (int)h, (int)r, R8, BH, strips, cparam, minv, fast_ok);
     return 0;
   }
-  dim3 block(32, 8), grid((w + 31) / 32, (h + 7) / 8, n < 65535u ? n : 65535u);
+  dim3 block(32, 8), grid((w + 31) / 32, min((h + 7) / 8, GRID_FRAMES), n < 65535u ? n : 65535u);
   GSB_LAUNCH(k_box_generic<ADAPTIVE>, grid, block, 0, s, dst, src, w, h, n, r, cparam);
   return 0;
 }
@@ -1170,9 +1173,10 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
         gsb::k_blur_sobel_tma<1>, gsb::k_blur_sobel_tma<2>, gsb::k_blur_sobel_tma<3>, gsb::k_blur_sobel_tma<4>,
         gsb::k_blur_sobel_tma<5>, gsb::k_blur_sobel_tma<6>, gsb::k_blur_sobel_tma<7>};
     const unsigned tiles_x = (w + gsb::BS_STRIDE - 1) / gsb::BS_STRIDE, tiles_y = (h + gsb::BS_TH - 1) / gsb::BS_TH;
-    GSB_ASSERT(tiles_y <= 65535u);
-    GSB_LAUNCH(blur_sobel_fn[radius - 1], dim3(tiles_x, tiles_y, n), gsb::BS_THREADS, gsb::BS_SMEM, s, tmap, dst, w, h);
-    return 0;
+    return gsb::for_row_groups(tiles_y, [&](unsigned t0, unsigned c) {
+      return gsb::launch(__FILE__, __LINE__, blur_sobel_fn[radius - 1], dim3(tiles_x, c, n), gsb::BS_THREADS, gsb::BS_SMEM, s,
+                         tmap, dst, w, h, t0);
+    });
   }
   // other radii / ragged widths: the two per-op kernels through a scratch frame batch (same result, 4 B/px)
   uint8_t *tmp = static_cast<uint8_t *>(gsb::workspace(s, gsb::WS_STAGE_FUSED, (size_t)w * h * n));

@@ -63,6 +63,16 @@ int for_frame_groups(unsigned n, F &&fn) {
   return 0;
 }
 
+// Row tiles meet the same limit within one frame.  A kernel that takes its row tile from blockIdx.y without a loop over
+// row tiles takes a tile-row offset t0 and works on row tile blockIdx.y + t0; for_row_groups calls fn(t0, count) for
+// each group of at most GRID_FRAMES tile rows, and fn launches count tile rows at offset t0.  Every launch still sees
+// the whole frame (its h, its tensor map), so halos and edge clipping are those of one launch.  A frame of at most
+// GRID_FRAMES row tiles is one launch at t0 = 0.
+template <class F>
+int for_row_groups(unsigned tiles_y, F &&fn) {
+  return for_frame_groups(tiles_y, static_cast<F &&>(fn));
+}
+
 // the reference's gs_assert (grayskull.h:94-98): message + abort
 #define GSB_ASSERT(cond)                                \
   do {                                                  \

@@ -190,22 +190,22 @@ __global__ void __launch_bounds__(256)
 k_fast_score(const uint8_t *__restrict__ src, unsigned w, unsigned h, unsigned n, uint8_t *__restrict__ score,
              unsigned sw, unsigned sh, unsigned t) {
   const unsigned x = 3 + blockIdx.x * 32 + threadIdx.x;
-  const unsigned y = 3 + blockIdx.y * 8 + threadIdx.y;
-  if (x + 3 >= w || y + 3 >= h) return;
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint8_t *c = src + (size_t)f * w * h + (size_t)y * w + x;
-    const unsigned p = __ldg(c), hi = p + t;
-    const bool wrap = t > p;          // reference :498: p - threshold wraps => always "darker"
-    const unsigned lo = p - t;        // only meaningful when !wrap
-    const int iw = (int)w;
-    // compass pre-test: any 9-arc contains at least two of ring positions 0, 4, 8, 12
-    unsigned v0 = __ldg(c - 3 * iw), v4 = __ldg(c + 3), v8 = __ldg(c + 3 * iw), v12 = __ldg(c - 3);
-    unsigned nb = (v0 > hi) + (v4 > hi) + (v8 > hi) + (v12 > hi);
-    unsigned nd = (!(v0 > hi) && (wrap || v0 < lo)) + (!(v4 > hi) && (wrap || v4 < lo)) +
-                  (!(v8 > hi) && (wrap || v8 < lo)) + (!(v12 > hi) && (wrap || v12 < lo));
-    unsigned s = 0;
-    if (nb >= 2 || nd >= 2) {
-      unsigned bright = 0, dark = 0, mind = 255;
+  if (x + 3 >= w) return;
+  for (unsigned y = 3 + blockIdx.y * 8 + threadIdx.y; y + 3 < h; y += gridDim.y * 8) {   // grid y: <= 65535 row tiles
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint8_t *c = src + (size_t)f * w * h + (size_t)y * w + x;
+      const unsigned p = __ldg(c), hi = p + t;
+      const bool wrap = t > p;          // reference :498: p - threshold wraps => always "darker"
+      const unsigned lo = p - t;        // only meaningful when !wrap
+      const int iw = (int)w;
+      // compass pre-test: any 9-arc contains at least two of ring positions 0, 4, 8, 12
+      unsigned v0 = __ldg(c - 3 * iw), v4 = __ldg(c + 3), v8 = __ldg(c + 3 * iw), v12 = __ldg(c - 3);
+      unsigned nb = (v0 > hi) + (v4 > hi) + (v8 > hi) + (v12 > hi);
+      unsigned nd = (!(v0 > hi) && (wrap || v0 < lo)) + (!(v4 > hi) && (wrap || v4 < lo)) +
+                    (!(v8 > hi) && (wrap || v8 < lo)) + (!(v12 > hi) && (wrap || v12 < lo));
+      unsigned s = 0;
+      if (nb >= 2 || nd >= 2) {
+        unsigned bright = 0, dark = 0, mind = 255;
 #define FAST_TAP(i, dx, dy)                                        \
   {                                                                \
     const unsigned v = __ldg(c + (dy) * iw + (dx));                \
@@ -215,11 +215,12 @@ k_fast_score(const uint8_t *__restrict__ src, unsigned w, unsigned h, unsigned n
     dark |= (unsigned)d << (i);                                    \
     mind = min(mind, v > p ? v - p : p - v);                       \
   }
-      FAST_RING(FAST_TAP)
+        FAST_RING(FAST_TAP)
 #undef FAST_TAP
-      if (run9(bright) || run9(dark)) s = mind;
+        if (run9(bright) || run9(dark)) s = mind;
+      }
+      if (x < sw && y < sh) score[(size_t)f * sw * sh + (size_t)y * sw + x] = (uint8_t)s;
     }
-    if (x < sw && y < sh) score[(size_t)f * sw * sh + (size_t)y * sw + x] = (uint8_t)s;
   }
 }
 
@@ -282,14 +283,14 @@ template <bool TMA>
 __global__ void __launch_bounds__(F2_THREADS)
 k_fast_tiled2(const __grid_constant__ CUtensorMap tmap, const uint8_t *__restrict__ src, unsigned w, unsigned h,
               uint8_t *__restrict__ score, unsigned t, unsigned mw, unsigned *__restrict__ masks,
-              unsigned *__restrict__ rowcount) {
+              unsigned *__restrict__ rowcount, unsigned ty0 /* first row tile of the launch: for_row_groups */) {
   __shared__ __align__(128) uint8_t s_src[F2_SH * FT_SW];
   __shared__ __align__(8) uint64_t bar;
   __shared__ __align__(16) uint8_t s_score[F2_ROWS * F2_PITCH];
   __shared__ uint16_t s_list[F2_ROWS * 130];       // candidate = (row << 8) | (column + 4)
   __shared__ unsigned s_cnt;
   const unsigned f = blockIdx.z, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int x0 = blockIdx.x * FT_W, y0 = 3 + blockIdx.y * F2_TH;   // tile = columns [x0, x0+128), rows [y0, y0+64)
+  const int x0 = blockIdx.x * FT_W, y0 = 3 + (blockIdx.y + ty0) * F2_TH;   // tile = columns [x0, x0+128), rows [y0, y0+64)
   const int iw = (int)w, ih = (int)h, ti = (int)min(t, 255u);
   const uint8_t *img = src + (size_t)f * w * h;
   if (tid == 0) s_cnt = 0;
@@ -956,18 +957,20 @@ static int fast_impl(const uint8_t *src, unsigned w, unsigned h, unsigned n, uin
   // huge t) take the literal per-pixel kernel: the tiled kernel's 16-bit lane arithmetic assumes t <= 255
   if (sw == w && sh == h && !force_generic() && threshold <= 255u) {
     // score + NMS mask in one kernel (k_fast_tiled2); the per-row counts are accumulated with atomics
-    dim3 grid((w + FT_W - 1) / FT_W, (h - 6 + F2_TH - 1) / F2_TH, n);
-    GSB_ASSERT(grid.y <= 65535u);
+    const unsigned tiles_x = (w + FT_W - 1) / FT_W, tiles_y = (h - 6 + F2_TH - 1) / F2_TH;
     GSB_CHECK(cudaMemsetAsync(rowcount, 0, sizeof(unsigned) * (size_t)rows * n, s));
     CUtensorMap tmap;
     const bool tiled = tma_ok(src, w) && tma_ok(score, w) && make_tmap_u8frames(&tmap, src, w, h, n, FT_SW / 4, F2_SH);
     if (!tiled) memset(&tmap, 0, sizeof(tmap));
-    GSB_LAUNCH(tiled ? k_fast_tiled2<true> : k_fast_tiled2<false>, grid, F2_THREADS, 0, s, tmap, src, w, h, score, threshold,
-               mw, masks, rowcount);
+    if (int rc = for_row_groups(tiles_y, [&](unsigned t0, unsigned c) {
+          return launch(__FILE__, __LINE__, tiled ? k_fast_tiled2<true> : k_fast_tiled2<false>, dim3(tiles_x, c, n), F2_THREADS, 0,
+                        s, tmap, src, w, h, score, threshold, mw, masks, rowcount, t0);
+        }))
+      return rc;
   } else {
     // foreign-sized score map (single-image gs_fast only), force_generic or t > 255: gs_set semantics per pixel,
     // then the NMS mask as a second pass
-    dim3 block(32, 8), grid((w - 6 + 31) / 32, (h - 6 + 7) / 8, n);
+    dim3 block(32, 8), grid((w - 6 + 31) / 32, min((h - 6 + 7) / 8, GRID_FRAMES), n);
     GSB_LAUNCH(k_fast_score, grid, block, 0, s, src, w, h, n, score, sw, sh, threshold);
     const bool words = sw % 4 == 0 && reinterpret_cast<uintptr_t>(score) % 4 == 0 && sw >= w && sh >= h;   // word pre-test stays inside the map
     GSB_LAUNCH(words ? k_nms_mask<true> : k_nms_mask<false>, dim3((rows + 7) / 8, n), 256, 0, s, score, sw, sh, w, h, mw, masks,

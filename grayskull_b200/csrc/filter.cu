@@ -37,9 +37,9 @@ constexpr int F3_ROWS = 16;
 template <bool NORM1>
 __global__ void __launch_bounds__(256)
 k_filter3(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, unsigned w, unsigned h, unsigned n,
-          uint32_t k0, uint32_t k1, uint32_t k2, uint32_t magic) {
+          uint32_t k0, uint32_t k1, uint32_t k2, uint32_t magic, unsigned ty0 /* first row tile of the launch: for_row_groups */) {
   const unsigned x = (blockIdx.x * 32 + (threadIdx.x & 31)) * 8;
-  const unsigned yb = (blockIdx.y * 8 + (threadIdx.x >> 5)) * F3_ROWS;
+  const unsigned yb = ((blockIdx.y + ty0) * 8 + (threadIdx.x >> 5)) * F3_ROWS;
   if (x >= w || yb >= h) return;
   for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
     const uint8_t *s = src + (size_t)f * w * h;
@@ -87,21 +87,23 @@ k_filter3(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, unsigned w
 __global__ void __launch_bounds__(256)
 k_filter_generic(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, unsigned w, unsigned h, unsigned n,
                  const int8_t *__restrict__ kern, unsigned kw, unsigned kh, unsigned norm) {
-  const unsigned x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (x >= w || y >= h) return;
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint8_t *s = src + (size_t)f * w * h;
-    int sum = 0;
-    for (unsigned j = 0; j < kh; j++) {
-      const unsigned sy = y + j - kh / 2;            // unsigned wrap == out of bounds, like gs_get
-      if (sy >= h) continue;
-      for (unsigned i = 0; i < kw; i++) {
-        const unsigned sx = x + i - kw / 2;
-        if (sx < w) sum += (int)__ldg(s + (size_t)sy * w + sx) * (int)__ldg(kern + j * kw + i);
+  const unsigned x = blockIdx.x * 32 + (threadIdx.x & 31);
+  if (x >= w) return;
+  for (unsigned y = blockIdx.y * 8 + (threadIdx.x >> 5); y < h; y += gridDim.y * 8) {   // grid y: <= 65535 row tiles
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint8_t *s = src + (size_t)f * w * h;
+      int sum = 0;
+      for (unsigned j = 0; j < kh; j++) {
+        const unsigned sy = y + j - kh / 2;            // unsigned wrap == out of bounds, like gs_get
+        if (sy >= h) continue;
+        for (unsigned i = 0; i < kw; i++) {
+          const unsigned sx = x + i - kw / 2;
+          if (sx < w) sum += (int)__ldg(s + (size_t)sy * w + sx) * (int)__ldg(kern + j * kw + i);
+        }
       }
+      const int v = (int)((unsigned)sum / norm);
+      dst[(size_t)f * w * h + (size_t)y * w + x] = (uint8_t)min(255, max(0, v));
     }
-    const int v = (int)((unsigned)sum / norm);
-    dst[(size_t)f * w * h + (size_t)y * w + x] = (uint8_t)min(255, max(0, v));
   }
 }
 
@@ -129,34 +131,35 @@ k_match_template(uint8_t *__restrict__ result, const uint8_t *__restrict__ img, 
                  const uint32_t *__restrict__ tpack, unsigned tw, unsigned th, unsigned twords) {
   const unsigned rw = w - tw + 1, rh = h - th + 1, wwords = w / 4;
   const unsigned cx = blockIdx.x * 32 + (threadIdx.x & 31);       // word column: results 4*cx .. 4*cx+3
-  const unsigned ry = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (4 * cx >= rw || ry >= rh) return;
+  if (4 * cx >= rw) return;
   const uint32_t tail_mask = (tw & 3) ? (0xFFFFFFFFu >> (8 * (4 - (tw & 3)))) : 0xFFFFFFFFu;
   const unsigned long long max_diff = (unsigned long long)tw * th * 255ull * 255ull;
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint32_t *base = reinterpret_cast<const uint32_t *>(img + (size_t)f * w * h);
-    unsigned long long tot0 = 0, tot1 = 0, tot2 = 0, tot3 = 0;
-    for (unsigned ty = 0; ty < th; ty++) {
-      const uint32_t *row = base + (size_t)(ry + ty) * wwords;
-      const uint32_t *trow = tpack + (size_t)ty * twords;
-      uint32_t s0 = 0, s1 = 0, s2 = 0, s3 = 0;
-      uint32_t A = __ldg(row + cx);
-      for (unsigned k = 0; k < twords; k++) {
-        const uint32_t B = cx + k + 1 < wwords ? __ldg(row + cx + k + 1) : 0u;
-        const uint32_t T = __ldg(trow + k);
-        uint32_t d0 = __vabsdiffu4(A, T), d1 = __vabsdiffu4(__funnelshift_r(A, B, 8), T);
-        uint32_t d2 = __vabsdiffu4(__funnelshift_r(A, B, 16), T), d3 = __vabsdiffu4(__funnelshift_r(A, B, 24), T);
-        if (k + 1 == twords) d0 &= tail_mask, d1 &= tail_mask, d2 &= tail_mask, d3 &= tail_mask;
-        s0 = dp4a_uu(d0, d0, s0), s1 = dp4a_uu(d1, d1, s1), s2 = dp4a_uu(d2, d2, s2), s3 = dp4a_uu(d3, d3, s3);
-        A = B;
+  for (unsigned ry = blockIdx.y * 8 + (threadIdx.x >> 5); ry < rh; ry += gridDim.y * 8) {   // grid y: <= 65535 row tiles
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint32_t *base = reinterpret_cast<const uint32_t *>(img + (size_t)f * w * h);
+      unsigned long long tot0 = 0, tot1 = 0, tot2 = 0, tot3 = 0;
+      for (unsigned ty = 0; ty < th; ty++) {
+        const uint32_t *row = base + (size_t)(ry + ty) * wwords;
+        const uint32_t *trow = tpack + (size_t)ty * twords;
+        uint32_t s0 = 0, s1 = 0, s2 = 0, s3 = 0;
+        uint32_t A = __ldg(row + cx);
+        for (unsigned k = 0; k < twords; k++) {
+          const uint32_t B = cx + k + 1 < wwords ? __ldg(row + cx + k + 1) : 0u;
+          const uint32_t T = __ldg(trow + k);
+          uint32_t d0 = __vabsdiffu4(A, T), d1 = __vabsdiffu4(__funnelshift_r(A, B, 8), T);
+          uint32_t d2 = __vabsdiffu4(__funnelshift_r(A, B, 16), T), d3 = __vabsdiffu4(__funnelshift_r(A, B, 24), T);
+          if (k + 1 == twords) d0 &= tail_mask, d1 &= tail_mask, d2 &= tail_mask, d3 &= tail_mask;
+          s0 = dp4a_uu(d0, d0, s0), s1 = dp4a_uu(d1, d1, s1), s2 = dp4a_uu(d2, d2, s2), s3 = dp4a_uu(d3, d3, s3);
+          A = B;
+        }
+        tot0 += s0, tot1 += s1, tot2 += s2, tot3 += s3;
       }
-      tot0 += s0, tot1 += s1, tot2 += s2, tot3 += s3;
+      uint8_t *o = result + (size_t)f * rw * rh + (size_t)ry * rw + 4 * cx;
+      o[0] = template_score(tot0, max_diff);
+      if (4 * cx + 1 < rw) o[1] = template_score(tot1, max_diff);
+      if (4 * cx + 2 < rw) o[2] = template_score(tot2, max_diff);
+      if (4 * cx + 3 < rw) o[3] = template_score(tot3, max_diff);
     }
-    uint8_t *o = result + (size_t)f * rw * rh + (size_t)ry * rw + 4 * cx;
-    o[0] = template_score(tot0, max_diff);
-    if (4 * cx + 1 < rw) o[1] = template_score(tot1, max_diff);
-    if (4 * cx + 2 < rw) o[2] = template_score(tot2, max_diff);
-    if (4 * cx + 3 < rw) o[3] = template_score(tot3, max_diff);
   }
 }
 
@@ -164,20 +167,22 @@ __global__ void __launch_bounds__(256)
 k_match_template_generic(uint8_t *__restrict__ result, const uint8_t *__restrict__ img, unsigned w, unsigned h, unsigned n,
                          const uint8_t *__restrict__ tmpl, unsigned tw, unsigned th) {
   const unsigned rw = w - tw + 1, rh = h - th + 1;
-  const unsigned rx = blockIdx.x * 32 + (threadIdx.x & 31), ry = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (rx >= rw || ry >= rh) return;
+  const unsigned rx = blockIdx.x * 32 + (threadIdx.x & 31);
+  if (rx >= rw) return;
   const unsigned long long max_diff = (unsigned long long)tw * th * 255ull * 255ull;
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint8_t *s = img + (size_t)f * w * h;
-    unsigned long long tot = 0;
-    for (unsigned ty = 0; ty < th; ty++) {
-      const uint8_t *p = s + (size_t)(ry + ty) * w + rx, *q = tmpl + (size_t)ty * tw;
-      for (unsigned tx = 0; tx < tw; tx++) {
-        const int diff = (int)__ldg(p + tx) - (int)__ldg(q + tx);
-        tot += (unsigned long long)(diff * diff);
+  for (unsigned ry = blockIdx.y * 8 + (threadIdx.x >> 5); ry < rh; ry += gridDim.y * 8) {   // grid y: <= 65535 row tiles
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint8_t *s = img + (size_t)f * w * h;
+      unsigned long long tot = 0;
+      for (unsigned ty = 0; ty < th; ty++) {
+        const uint8_t *p = s + (size_t)(ry + ty) * w + rx, *q = tmpl + (size_t)ty * tw;
+        for (unsigned tx = 0; tx < tw; tx++) {
+          const int diff = (int)__ldg(p + tx) - (int)__ldg(q + tx);
+          tot += (unsigned long long)(diff * diff);
+        }
       }
+      result[(size_t)f * rw * rh + (size_t)ry * rw + rx] = template_score(tot, max_diff);
     }
-    result[(size_t)f * rw * rh + (size_t)ry * rw + rx] = template_score(tot, max_diff);
   }
 }
 
@@ -262,12 +267,12 @@ int gs_b200_filter_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned 
     }
     const bool magic_ok = norm >= 2 && pos * norm < (1ull << 32) && ((1ull << 32) - neg) / norm >= 256;
     if (norm == 1 || magic_ok) {
-      dim3 grid((w / 8 + 31) / 32, (h + 8 * gsb::F3_ROWS - 1) / (8 * gsb::F3_ROWS), zn);
-      GSB_ASSERT(grid.y <= 65535u);
+      const unsigned tiles_y = (h + 8 * gsb::F3_ROWS - 1) / (8 * gsb::F3_ROWS);
       const uint32_t magic = norm == 1 ? 0 : (uint32_t)((1ull << 32) / norm + 1);
-      GSB_LAUNCH(norm == 1 ? gsb::k_filter3<true> : gsb::k_filter3<false>, grid, 256, 0, st, dst, src, w, h, n, kr[0], kr[1],
-                 kr[2], magic);
-      return 0;
+      return gsb::for_row_groups(tiles_y, [&](unsigned t0, unsigned c) {
+        return gsb::launch(__FILE__, __LINE__, norm == 1 ? gsb::k_filter3<true> : gsb::k_filter3<false>,
+                           dim3((w / 8 + 31) / 32, c, zn), 256, 0, st, dst, src, w, h, n, kr[0], kr[1], kr[2], magic, t0);
+      });
     }
   }
   const size_t kbytes = has_kernel ? (size_t)kw * kh : 0;
@@ -280,8 +285,7 @@ int gs_b200_filter_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsigned 
   int8_t *dk = static_cast<int8_t *>(gsb::workspace(st, gsb::WS_HIST, kbytes + 16));
   if (!dk) return gsb::workspace_error();
   if (kbytes) GSB_CHECK(cudaMemcpyAsync(dk, kernel, kbytes, cudaMemcpyHostToDevice, st));
-  dim3 grid((w + 31) / 32, (h + 7) / 8, zn);
-  GSB_ASSERT(grid.y <= 65535u);
+  dim3 grid((w + 31) / 32, min((h + 7) / 8, gsb::GRID_FRAMES), zn);
   GSB_LAUNCH(gsb::k_filter_generic, grid, 256, 0, st, dst, src, w, h, n, dk, has_kernel ? kw : 0, has_kernel ? kh : 0, norm);
   return 0;
 }
@@ -299,12 +303,10 @@ int gs_b200_match_template_batch(uint8_t *result, const uint8_t *img, unsigned w
     uint32_t *tpack = static_cast<uint32_t *>(gsb::workspace(st, gsb::WS_HIST, sizeof(uint32_t) * (size_t)twords * th));
     if (!tpack) return gsb::workspace_error();
     GSB_LAUNCH(gsb::k_pack_template, (twords * th + 255) / 256, 256, 0, st, tpack, tmpl, tw, th, twords);
-    dim3 grid(((rw + 3) / 4 + 31) / 32, (rh + 7) / 8, zn);
-    GSB_ASSERT(grid.y <= 65535u);
+    dim3 grid(((rw + 3) / 4 + 31) / 32, min((rh + 7) / 8, gsb::GRID_FRAMES), zn);
     GSB_LAUNCH(gsb::k_match_template, grid, 256, 0, st, result, img, w, h, n, tpack, tw, th, twords);
   } else {
-    dim3 grid((rw + 31) / 32, (rh + 7) / 8, zn);
-    GSB_ASSERT(grid.y <= 65535u);
+    dim3 grid((rw + 31) / 32, min((rh + 7) / 8, gsb::GRID_FRAMES), zn);
     GSB_LAUNCH(gsb::k_match_template_generic, grid, 256, 0, st, result, img, w, h, n, tmpl, tw, th);
   }
   return 0;

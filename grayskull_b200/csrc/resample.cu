@@ -10,31 +10,33 @@ namespace gsb {
 __global__ void k_downsample_vec(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src, unsigned sw,
                                  unsigned sh, unsigned dw, unsigned dh, unsigned n) {
   const unsigned gx = blockIdx.x * blockDim.x + threadIdx.x;  // 8 dst pixels each
-  const unsigned y = blockIdx.y;
   if (gx * 8 >= dw) return;
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint4 *r0 = reinterpret_cast<const uint4 *>(src + (size_t)f * sw * sh + (size_t)(2 * y) * sw) + gx;
-    const uint4 *r1 = reinterpret_cast<const uint4 *>(src + (size_t)f * sw * sh + (size_t)(2 * y + 1) * sw) + gx;
-    const uint4 a = __ldg(r0), b = __ldg(r1);
-    auto quad = [](uint32_t u, uint32_t v) -> uint32_t {  // lanes: (b0+b1+.., b2+b3+..) >> 2
-      uint32_t s = (u & 0x00FF00FFu) + ((u >> 8) & 0x00FF00FFu) + (v & 0x00FF00FFu) + ((v >> 8) & 0x00FF00FFu);
-      return (s >> 2) & 0x00FF00FFu;
-    };
-    uint2 o;
-    o.x = prmt(quad(a.x, b.x), quad(a.y, b.y), 0x6420);
-    o.y = prmt(quad(a.z, b.z), quad(a.w, b.w), 0x6420);
-    st_cs_u2(dst + (size_t)f * dw * dh + (size_t)y * dw + gx * 8, o);
+  for (unsigned y = blockIdx.y; y < dh; y += gridDim.y) {      // grid y: <= 65535 rows
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint4 *r0 = reinterpret_cast<const uint4 *>(src + (size_t)f * sw * sh + (size_t)(2 * y) * sw) + gx;
+      const uint4 *r1 = reinterpret_cast<const uint4 *>(src + (size_t)f * sw * sh + (size_t)(2 * y + 1) * sw) + gx;
+      const uint4 a = __ldg(r0), b = __ldg(r1);
+      auto quad = [](uint32_t u, uint32_t v) -> uint32_t {  // lanes: (b0+b1+.., b2+b3+..) >> 2
+        uint32_t s = (u & 0x00FF00FFu) + ((u >> 8) & 0x00FF00FFu) + (v & 0x00FF00FFu) + ((v >> 8) & 0x00FF00FFu);
+        return (s >> 2) & 0x00FF00FFu;
+      };
+      uint2 o;
+      o.x = prmt(quad(a.x, b.x), quad(a.y, b.y), 0x6420);
+      o.y = prmt(quad(a.z, b.z), quad(a.w, b.w), 0x6420);
+      st_cs_u2(dst + (size_t)f * dw * dh + (size_t)y * dw + gx * 8, o);
+    }
   }
 }
 
 __global__ void k_downsample_generic(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src,
                                      unsigned sw, unsigned sh, unsigned dw, unsigned dh, unsigned n) {
   const unsigned x = blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= dw || y >= dh) return;
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint8_t *p = src + (size_t)f * sw * sh + (size_t)(2 * y) * sw + 2 * x;
-    dst[(size_t)f * dw * dh + (size_t)y * dw + x] = (uint8_t)((p[0] + p[1] + p[sw] + p[sw + 1]) / 4);
+  if (x >= dw) return;
+  for (unsigned y = blockIdx.y * blockDim.y + threadIdx.y; y < dh; y += gridDim.y * blockDim.y) {   // grid y: <= 65535 row tiles
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint8_t *p = src + (size_t)f * sw * sh + (size_t)(2 * y) * sw + 2 * x;
+      dst[(size_t)f * dw * dh + (size_t)y * dw + x] = (uint8_t)((p[0] + p[1] + p[sw] + p[sw + 1]) / 4);
+    }
   }
 }
 
@@ -66,12 +68,12 @@ __device__ __forceinline__ uint32_t f_trunc_bits(float p) { return __float_as_ui
 template <bool VEC>
 __global__ void __launch_bounds__(256)
 k_resize(uint8_t *__restrict__ dst, unsigned dw, unsigned dh, const uint8_t *__restrict__ src, unsigned sw,
-         unsigned sh, unsigned n, bool src_aligned8) {
+         unsigned sh, unsigned n, bool src_aligned8, unsigned ty0 /* first row tile of the launch: for_row_groups */) {
   // the y-axis coefficients (an IEEE division each) of the CTA's 64 rows: once per CTA, not once per thread and row
   __shared__ unsigned s_y0[8 * RS_ROWS], s_y1[8 * RS_ROWS];
   __shared__ float s_dy[8 * RS_ROWS], s_omy[8 * RS_ROWS];   // pre-scaled y weights
   if (threadIdx.x < 8 * RS_ROWS) {
-    const unsigned yy = blockIdx.y * 8 * RS_ROWS + threadIdx.x;
+    const unsigned yy = (blockIdx.y + ty0) * 8 * RS_ROWS + threadIdx.x;
     unsigned a = 0, b = 0;
     float fr = 0.0f;
     if (yy < dh) resize_axis(yy, sh, dh, a, b, fr);
@@ -80,7 +82,7 @@ k_resize(uint8_t *__restrict__ dst, unsigned dw, unsigned dh, const uint8_t *__r
   }
   __syncthreads();
   const unsigned x = (blockIdx.x * 32 + (threadIdx.x & 31)) * 4;
-  const unsigned yb = (blockIdx.y * 8 + (threadIdx.x >> 5)) * RS_ROWS;
+  const unsigned yb = ((blockIdx.y + ty0) * 8 + (threadIdx.x >> 5)) * RS_ROWS;
   if (x >= dw || yb >= dh) return;
   const unsigned yl = (threadIdx.x >> 5) * RS_ROWS;       // this warp's first row in the table
   unsigned x0[4], x1[4];
@@ -140,14 +142,15 @@ constexpr int RT_MAX_BYTES = 64 * 1024;
 template <bool VEC>
 __global__ void __launch_bounds__(256)
 k_resize_tiled(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, unsigned dw, unsigned dh, unsigned sw,
-               unsigned sh, unsigned n, unsigned pitch /* bytes, multiple of 16 = the TMA box width */, unsigned max_rows) {
+               unsigned sh, unsigned n, unsigned pitch /* bytes, multiple of 16 = the TMA box width */, unsigned max_rows,
+               unsigned ty0 /* first row tile of the launch: for_row_groups */) {
   extern __shared__ __align__(128) uint8_t s_tile[];
   __shared__ __align__(8) uint64_t bar;
   __shared__ unsigned s_roff[8 * RS_ROWS];           // byte offset of source row y0 in the staged rectangle
   __shared__ float s_dy[8 * RS_ROWS], s_omy[8 * RS_ROWS];   // pre-scaled y weights
   __shared__ unsigned s_reg[2];                      // cxa (first staged column, 16-aligned), cya (first staged row)
   const unsigned tid = threadIdx.x;
-  const unsigned tx0 = blockIdx.x * 128, ty0 = blockIdx.y * 8 * RS_ROWS;
+  const unsigned tx0 = blockIdx.x * 128, y0 = (blockIdx.y + ty0) * 8 * RS_ROWS;
   if (tid == 0) {   // the mapping is monotonic: the tile's first / last pixel bound the rectangle
     unsigned a0, b0, a1, b1;
     float f;
@@ -155,8 +158,8 @@ k_resize_tiled(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ d
     resize_axis(min(tx0 + 127u, dw - 1), sw, dw, a1, b1, f);
     const unsigned cxa = a0 & ~15u;                  // the inner TMA coordinate must be a multiple of 16 bytes
     const unsigned cols = a1 + 2 - cxa;              // taps x0 and x0 + 1
-    resize_axis(ty0, sh, dh, a0, b0, f);
-    resize_axis(min(ty0 + 8u * RS_ROWS - 1, dh - 1), sh, dh, a1, b1, f);
+    resize_axis(y0, sh, dh, a0, b0, f);
+    resize_axis(min(y0 + 8u * RS_ROWS - 1, dh - 1), sh, dh, a1, b1, f);
     s_reg[0] = cxa, s_reg[1] = a0;
     if (cols > pitch || a1 + 2 - a0 > max_rows) __trap();   // the host's bound covers the tile (with spare); never silently wrong
     mbar_init(&bar, 1);
@@ -165,7 +168,7 @@ k_resize_tiled(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ d
   __syncthreads();
   const unsigned cxa = s_reg[0], cya = s_reg[1];
   if (tid < 8 * RS_ROWS) {
-    const unsigned yy = ty0 + tid;
+    const unsigned yy = y0 + tid;
     unsigned a = cya, b = 0;
     float fr = 0.0f;
     if (yy < dh) resize_axis(yy, sh, dh, a, b, fr);
@@ -173,7 +176,7 @@ k_resize_tiled(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ d
     s_dy[tid] = __fmul_rn(fr, RS_WY_SCALE), s_omy[tid] = __fmul_rn(__fsub_rn(1.0f, fr), RS_WY_SCALE);
   }
   const unsigned x = tx0 + (tid & 31) * 4;
-  const unsigned yl = (tid >> 5) * RS_ROWS, yb = ty0 + yl;
+  const unsigned yl = (tid >> 5) * RS_ROWS, yb = y0 + yl;
   // The second tap of each axis is read at x0 + 1 / y0 + 1 WITHOUT the reference's clamp: x0 == sw - 1 only when the
   // clamped coordinate is exactly sw - 1, i.e. dx == 0, and then whatever (finite) byte sits at x0 + 1 is multiplied
   // by zero; same for y.  (TMA zero-fills outside the image and the rectangle has the spare column / row.)
@@ -229,12 +232,12 @@ int gs_b200_downsample_batch(uint8_t *dst, const uint8_t *src, unsigned sw, unsi
   const unsigned dw = sw / 2, dh = sh / 2;
   if (n == 0 || dw == 0 || dh == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(s);
-  const unsigned zn = n < 65535u ? n : 65535u;
-  if (gsb::tma_ok(src, sw) && reinterpret_cast<uintptr_t>(dst) % 8 == 0 && dh <= 65535u) {
-    dim3 block(128), grid((dw / 8 + 127) / 128, dh, zn);
+  const unsigned zn = n < 65535u ? n : 65535u, gy = dh < gsb::GRID_FRAMES ? dh : gsb::GRID_FRAMES;
+  if (gsb::tma_ok(src, sw) && reinterpret_cast<uintptr_t>(dst) % 8 == 0) {
+    dim3 block(128), grid((dw / 8 + 127) / 128, gy, zn);
     GSB_LAUNCH(gsb::k_downsample_vec, grid, block, 0, st, dst, src, sw, sh, dw, dh, n);
   } else {
-    dim3 block(32, 8), grid((dw + 31) / 32, (dh + 7) / 8, zn);
+    dim3 block(32, 8), grid((dw + 31) / 32, min((dh + 7) / 8, gsb::GRID_FRAMES), zn);
     GSB_LAUNCH(gsb::k_downsample_generic, grid, block, 0, st, dst, src, sw, sh, dw, dh, n);
   }
   return 0;
@@ -251,8 +254,8 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
   if (sw == 2 * dw && sh == 2 * dh && (unsigned long long)(2 * dw) * dw < (1ull << 24) &&
       (unsigned long long)(2 * dh) * dh < (1ull << 24) && !gsb::force_generic())
     return gs_b200_downsample_batch(dst, src, sw, sh, n, s);
-  dim3 grid((dw + 127) / 128, (dh + 8 * gsb::RS_ROWS - 1) / (8 * gsb::RS_ROWS), n < gsb::GRID_FRAMES ? n : gsb::GRID_FRAMES);
-  GSB_ASSERT(grid.y <= 65535u);
+  const unsigned tiles_y = (dh + 8 * gsb::RS_ROWS - 1) / (8 * gsb::RS_ROWS);
+  dim3 grid((dw + 127) / 128, 1, n < gsb::GRID_FRAMES ? n : gsb::GRID_FRAMES);
   const bool aligned8 = sw % 8 == 0 && reinterpret_cast<uintptr_t>(src) % 8 == 0;   // every source row 8-byte aligned
   const bool vec_dst = dw % 4 == 0 && reinterpret_cast<uintptr_t>(dst) % 4 == 0;
   {
@@ -275,13 +278,19 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
       return gsb::for_frame_groups(n, [&](unsigned f0, unsigned c) {
         if (f0 && !group_map(f0, c)) return gsb::record_error(cudaErrorInvalidValue, __FILE__, __LINE__);
         grid.z = c;
-        return gsb::launch(__FILE__, __LINE__, vec_dst ? gsb::k_resize_tiled<true> : gsb::k_resize_tiled<false>, grid, 256, bytes,
-                           static_cast<cudaStream_t>(s), tm, dst + (size_t)f0 * dw * dh, dw, dh, sw, sh, c, pitch, rows);
+        return gsb::for_row_groups(tiles_y, [&](unsigned t0, unsigned cy) {
+          grid.y = cy;
+          return gsb::launch(__FILE__, __LINE__, vec_dst ? gsb::k_resize_tiled<true> : gsb::k_resize_tiled<false>, grid, 256,
+                             bytes, static_cast<cudaStream_t>(s), tm, dst + (size_t)f0 * dw * dh, dw, dh, sw, sh, c, pitch, rows,
+                             t0);
+        });
       });
     }
   }
-  GSB_LAUNCH(vec_dst ? gsb::k_resize<true> : gsb::k_resize<false>, grid, 256, 0, static_cast<cudaStream_t>(s), dst, dw, dh, src,
-             sw, sh, n, aligned8);
-  return 0;
+  return gsb::for_row_groups(tiles_y, [&](unsigned t0, unsigned cy) {
+    grid.y = cy;
+    return gsb::launch(__FILE__, __LINE__, vec_dst ? gsb::k_resize<true> : gsb::k_resize<false>, grid, 256, 0,
+                       static_cast<cudaStream_t>(s), dst, dw, dh, src, sw, sh, n, aligned8, t0);
+  });
 }
 }

@@ -169,28 +169,29 @@ template <int OP>
 __global__ void k_stencil3_generic(uint8_t *__restrict__ dst, const uint8_t *__restrict__ src,
                                    unsigned w, unsigned h, unsigned n) {
   const unsigned x = blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= w || y >= h) return;
-  for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
-    const uint8_t *s = src + (size_t)f * w * h;
-    uint8_t *d = dst + (size_t)f * w * h;
-    if (OP == OP_SOBEL) {
-      if (x == 0 || y == 0 || x + 1 >= w || y + 1 >= h) continue;
-      const uint8_t *a = s + (size_t)(y - 1) * w + x, *b = a + w, *c = b + w;
-      int gx = -a[-1] + a[1] - 2 * b[-1] + 2 * b[1] - c[-1] + c[1];
-      int gy = -a[-1] - 2 * a[0] - a[1] + c[-1] + 2 * c[0] + c[1];
-      int m = (abs(gx) + abs(gy)) / 2;
-      d[(size_t)y * w + x] = (uint8_t)min(m, 255);
-    } else {
-      int v = OP == OP_ERODE ? 255 : 0;
-      for (int dy = -1; dy <= 1; dy++)
-        for (int dx = -1; dx <= 1; dx++) {
-          int yy = (int)y + dy, xx = (int)x + dx;
-          if (yy < 0 || yy >= (int)h || xx < 0 || xx >= (int)w) continue;
-          int p = s[(size_t)yy * w + xx];
-          v = OP == OP_ERODE ? min(v, p) : max(v, p);
-        }
-      d[(size_t)y * w + x] = (uint8_t)v;
+  if (x >= w) return;
+  for (unsigned y = blockIdx.y * blockDim.y + threadIdx.y; y < h; y += gridDim.y * blockDim.y) {   // grid y: <= 65535 row tiles
+    for (unsigned f = blockIdx.z; f < n; f += gridDim.z) {
+      const uint8_t *s = src + (size_t)f * w * h;
+      uint8_t *d = dst + (size_t)f * w * h;
+      if (OP == OP_SOBEL) {
+        if (x == 0 || y == 0 || x + 1 >= w || y + 1 >= h) continue;
+        const uint8_t *a = s + (size_t)(y - 1) * w + x, *b = a + w, *c = b + w;
+        int gx = -a[-1] + a[1] - 2 * b[-1] + 2 * b[1] - c[-1] + c[1];
+        int gy = -a[-1] - 2 * a[0] - a[1] + c[-1] + 2 * c[0] + c[1];
+        int m = (abs(gx) + abs(gy)) / 2;
+        d[(size_t)y * w + x] = (uint8_t)min(m, 255);
+      } else {
+        int v = OP == OP_ERODE ? 255 : 0;
+        for (int dy = -1; dy <= 1; dy++)
+          for (int dx = -1; dx <= 1; dx++) {
+            int yy = (int)y + dy, xx = (int)x + dx;
+            if (yy < 0 || yy >= (int)h || xx < 0 || xx >= (int)w) continue;
+            int p = s[(size_t)yy * w + xx];
+            v = OP == OP_ERODE ? min(v, p) : max(v, p);
+          }
+        d[(size_t)y * w + x] = (uint8_t)v;
+      }
     }
   }
 }
@@ -207,7 +208,7 @@ static int launch_stencil3(uint8_t *dst, const uint8_t *src, unsigned w, unsigne
     GSB_ASSERT(blocks < 0x7FFFFFFFull);
     GSB_LAUNCH(k_stencil3_tma<OP>, (unsigned)blocks, S3_WARPS * 32, 0, s, tmap, dst, w, h, tiles_x, tiles_y);
   } else {
-    dim3 block(32, 8), grid((w + 31) / 32, (h + 7) / 8, n < 65535u ? n : 65535u);
+    dim3 block(32, 8), grid((w + 31) / 32, min((h + 7) / 8, GRID_FRAMES), n < 65535u ? n : 65535u);
     GSB_LAUNCH(k_stencil3_generic<OP>, grid, block, 0, s, dst, src, w, h, n);
   }
   return 0;

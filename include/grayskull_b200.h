@@ -10,6 +10,8 @@
  * The single-image gs_* functions are the n == 1 case plus staging and a stream sync.
  * The frame count n (npairs for gs_b200_match_orb_batch) is bounded only by device memory: batches above the
  * grid's 65535 limit run as consecutive frame groups on the same stream, on the same kernels as smaller ones.
+ * The frame height is bounded only by device memory, too: a frame of more than 65535 row tiles runs on the kernels a
+ * shorter frame of the same width takes, as launches of at most 65535 tile rows or as a loop over row tiles.
  *
  * Plain C99: only pointers, sizes and PODs cross this boundary.  Every function returns 0 on
  * success or a non-zero cudaError_t value (gs_b200_last_error() gives the text).  Argument
