@@ -47,8 +47,8 @@ def segments(x, k):
 
 
 def flat(x, k):
-    """k frames of a buffer -> its bytes as they lie on the device"""
-    return np.concatenate([s.reshape(-1) for s in segments(x, k)])
+    """k frames of a buffer -> its bytes as they lie on the device (none for a list of no segments: a 1-level pyramid)"""
+    return np.concatenate([np.zeros(0, np.uint8)] + [s.reshape(-1) for s in segments(x, k)])
 
 
 def unflat(b, per, k):
@@ -134,7 +134,7 @@ def spec(sym, g):
         f, it = getattr(lib, sym), g["iters"]
 
         def morph_n(a):
-            for _ in range(it):
+            for _ in range(min(it, max(w, h))):     # past max(w, h) - 1 passes the square covers the frame
                 a = L.o_morph(O, a, "dilate" in sym)
             return a
         return Spec(one, {"dst": px}, lambda P, n, s: f(P["dst"], P["src"], w, h, n, it, s),

@@ -16,7 +16,6 @@ dispatch geometry per row (op, sizes, a byte offset for each base) and the kerne
     a kernel added without a row fails without a GPU.
 """
 import os
-import re
 
 import numpy as np
 import pytest
@@ -185,25 +184,73 @@ def _other_rows():
             row("match_orb", ("gsb::k_match_best", "gsb::k_match_compact"), n=3)]
 
 
+def _morph_n_rows():
+    out = []
+    for op, k in (("erode_n", 1), ("dilate_n", 2)):
+        tma, s3 = "gsb::k_morph_tma<%d, %%d>" % k, "gsb::k_stencil3_tma<%d>" % k
+        rows_cols = ("gsb::k_morph_rows<%d>" % k, "gsb::k_morph_cols<%d>" % k)
+        # TMA geometry, 2 <= N <= 16: one launch of k_morph_tma<OP, N>
+        out += [row(op, tma % it, w=272, h=70, iters=it) for it in range(2, 17)]
+        # 17 <= N <= 48: launches of at most 16 composed through the workspace, a remainder of 1 on the 3x3 kernel
+        out += [row(op, (tma % 16, s3), w=272, h=70, iters=17),
+                row(op, (tma % 16, s3), w=272, h=70, iters=33),
+                row(op, tma % 16, w=272, h=70, iters=48)]
+        # the row and column passes: a ragged width, a base off 16 bytes, N' = max(min(N, w - 1), min(N, h - 1)) > 48
+        out += [row(op, rows_cols, w=100, h=70, iters=3),
+                row(op, rows_cols, w=272, h=70, iters=5, **({"src": 1} if k == 1 else {"dst": 1})),
+                row(op, rows_cols, w=272, h=70, iters=1000)]
+        # iters 1 is the 3x3 call; a saturating count clamps to N' = 271 (iters 0 is a device copy, no kernel)
+        out += [row(op, s3, w=272, h=70, iters=1),
+                row(op, rows_cols, w=272, h=70, iters=2 ** 32 - 1)]
+    return out
+
+
+def _roi_rows():
+    copy, gather = "gsb::k_roi_copy", "gsb::k_roi_gather<%d>"
+    # unscaled regions inside the frame take k_roi_copy in either mode, at any width, offset and alignment
+    return [row("crop_resize", copy, w=272, h=70, roi=(3, 5, 160, 40), dw=160, dh=40, mode=0),
+            row("crop_resize", copy, w=101, h=37, roi=(13, 7, 77, 29), dw=77, dh=29, mode=1, src=5, dst=3),
+            # scaled regions: the mode's gather kernel
+            row("crop_resize", gather % 0, w=272, h=70, roi=(7, 3, 50, 31), dw=64, dh=64, mode=0),
+            row("crop_resize", gather % 1, w=101, h=37, roi=(2, 1, 97, 35), dw=40, dh=13, mode=1, src=7, dst=2),
+            # device lists of unscaled and scaled regions: both kernels run over the list, each on its own slots
+            row("rois_resize", (copy, gather % 0), w=272, h=70, dw=64, dh=48, mode=0),
+            row("rois_resize", (copy, gather % 1), w=101, h=37, dw=33, dh=20, mode=1, src=3, dst=5)]
+
+
+def _pyramid_rows():
+    # the last level: FAST, the quota clamps around select, describe, then the merge of every level's list
+    last = ("gsb::k_pyr_quota", "gsb::k_pyr_merge", "gsb::k_row_scan", "gsb::k_nms_emit_masks", "gsb::k_orb_select",
+            "gsb::k_orb_moments", "gsb::k_orb_trig")
+    tiled, plain = "gsb::k_fast_tiled2<true>", "gsb::k_fast_tiled2<false>"
+    words, bytes_ = "gsb::k_orb_brief<true>", "gsb::k_orb_brief<false>"
+    down_vec, down_generic = "gsb::k_downsample_vec", "gsb::k_downsample_generic"
+    return [row("orb_pyramid", last + (tiled, words), w=272, h=70, levels=1),
+            # level 1 is 136 wide (8 mod 16): FAST on plain loads there
+            row("orb_pyramid", last + (tiled, plain, words, down_vec), w=272, h=70, levels=2),
+            # level 2 is made from the 136-wide level 1 by the generic downsample
+            row("orb_pyramid", last + (tiled, plain, words, down_vec, down_generic), w=272, h=140, levels=3),
+            row("orb_pyramid", last + (plain, bytes_, words, down_generic), w=272, h=70, levels=2, src=1)]
+
+
 ROWS = (_box_rows() + _blur_sobel_rows() + _stencil_rows() + _resample_rows() + _integral_rows() + _histogram_rows() +
-        _filter_rows() + _fast_orb_rows() + _lbp_rows() + _other_rows())
+        _filter_rows() + _fast_orb_rows() + _lbp_rows() + _other_rows() + _morph_n_rows() + _roi_rows() +
+        _pyramid_rows())
 
 # kernels without a row here, each with the reason
 ALLOWED = {
-    r"gsb::k_trig_selfcheck": "runs once per process on its own stream before the first ORB angle; "
-                              "test_gpu_parity.py::test_trig_selfcheck_matches_this_libm checks its verdict",
-    r"gsb::k_orient_one": "single-image gs_compute_orientation; test_gpu_parity.py golden and large-radius tests",
-    r"gsb::k_brief_one": "single-image gs_brief_descriptor; test_gpu_parity.py golden test",
-    r"gsb::k_lbp_window_one": "single-image gs_lbp_window; test_gpu_parity.py golden test",
-    r"gsb::k_morph_(tma|rows|cols)<.*>": "erode_n / dilate_n: test_morph_iter.py runs both of its paths at pointer "
-                                        "offsets and counts their launches",
-    r"gsb::k_roi_.*": "region calls: test_roi.py's DISPATCH census and its witnessed GPU cases cover every one",
-    r"gsb::k_pyr_.*": "pyramid ORB: test_orb_pyramid.py's DISPATCH census and its witnessed GPU cases cover every one",
+    "gsb::k_trig_selfcheck": "runs once per process on its own stream before the first ORB angle; "
+                             "test_gpu_parity.py::test_trig_selfcheck_matches_this_libm checks its verdict",
+    "gsb::k_orient_one": "single-image gs_compute_orientation; test_gpu_parity.py golden and large-radius tests",
+    "gsb::k_brief_one": "single-image gs_brief_descriptor; test_gpu_parity.py golden test",
+    "gsb::k_lbp_window_one": "single-image gs_lbp_window; test_gpu_parity.py golden test",
 }
 
 
 def row_id(op, p):
-    return "-".join([op] + ["%s%s" % (k, v) for k, v in p.items() if k != "n"] + ["n%d" % p["n"]])
+    def text(v):
+        return "_".join(map(str, v)) if isinstance(v, tuple) else v
+    return "-".join([op] + ["%s%s" % (k, text(v)) for k, v in p.items() if k != "n"] + ["n%d" % p["n"]])
 
 
 # ---- CPU: the census -----------------------------------------------------------------------------------------------
@@ -220,9 +267,10 @@ def test_every_kernel_has_a_row():
     built = set(L.sass_functions())
     assert len(built) > 50, sorted(built)
     table = {kernel_id(k) for _, kernels, _ in ROWS for k in kernels}
-    orphans = sorted(k for k in built if k not in table and not any(re.fullmatch(a, k) for a in ALLOWED))
+    orphans = sorted(built - table - set(ALLOWED))
     assert not orphans, "kernels with neither a dispatch row nor an ALLOWED entry: %s" % orphans
     assert not sorted(table - built), "rows naming kernels the library does not have: %s" % sorted(table - built)
+    assert not sorted(set(ALLOWED) - built), "ALLOWED names kernels the library does not have"
     assert not [k for k in built if k.startswith("gsb::k_box_wide<") and k.count(",")], "k_box_wide has one parameter"
 
 
@@ -274,7 +322,14 @@ OPS = {
     "blob_corners": ("gs_b200_blob_corners", dict(labels=2)),
     "perspective": ("gs_b200_perspective_correct_batch", dict(per_frame=0)),
     "match_orb": ("gs_b200_match_orb_batch", dict(s1=130, s2=90, mm=150)),
+    "erode_n": ("gs_b200_erode_n_batch", {}),
+    "dilate_n": ("gs_b200_dilate_n_batch", {}),
+    "crop_resize": ("gs_b200_crop_resize_batch", {}),
+    "rois_resize": ("gs_b200_rois_resize_batch", dict(mr=5)),
+    "orb_pyramid": ("gs_b200_orb_pyramid_batch", dict(nkps=400, t=20)),
 }
+# ops whose rows run on _calls.inputs' real inputs: region lists of unscaled and scaled slots, random score maps
+DEFAULT_INPUTS = {"erode_n", "dilate_n", "crop_resize", "rois_resize", "orb_pyramid"}
 
 
 def _cascade(kind):
@@ -291,6 +346,8 @@ def _cascade(kind):
 def row_inputs(O, op, g):
     """{buffer: its n frames} of a row"""
     w, h, n = g.get("w"), g.get("h"), g["n"]
+    if op in DEFAULT_INPUTS:
+        return calls.inputs(OPS[op][0], g, n, 1)
     if op == "find_best_match":
         # result maps with odd rw * rh: frame bases fall mid-word; winners in a chunk's unaligned head and tail
         px = w * h
@@ -361,7 +418,7 @@ def run_row(lib, O, op, p):
     for b, r in R.items():
         got, exp = r.read(b), calls.flat(want[b], n) if b in want else dict(bufs)[b]
         assert np.array_equal(got, exp), "%s: byte %d of %d differs" % (b, int(np.argmax(got != exp)), got.size)
-    if op in ("fast", "orb"):
+    if op in ("fast", "orb", "orb_pyramid"):
         assert want["counts"].sum() > 0 or g["t"] > 255
     if op == "lbp":
         assert want["counts"].sum() > 0

@@ -3,14 +3,13 @@ multi-scale ORB: extract_pyramid_orb_nm of its `orb` verb.
 
 pyramid_orb() (tests/_libs.py) restates that helper from its behaviour on the oracle's gso_downsample / gso_orb_extract, with its
 one buffer (pyramid levels 1..L-1, then score maps 0..L-1) as a numpy array; orb_verb_line() restates the verb's
-printed line, the 1 MiB buffer it shares between the template and the scene included.  DISPATCH is the coverage record
-of the pyramid's own kernels (gsb::k_pyr_*): every one of them in the library's SASS, with the cases that must launch
-it.  test_host_logic.py checks the exports and the binding table, test_streams.py the runtime calls of pyramid.o, and
-test_dispatch_paths.py that its launches go through gsb::launch.
+printed line, the 1 MiB buffer it shares between the template and the scene included.  test_dispatch_paths.py has the
+rows that pick each kernel of the call, the pyramid's own (gsb::k_pyr_*) included, and checks that its launches go
+through gsb::launch; test_host_logic.py checks the exports, the binding table and that every kernel is sm_90a,
+test_streams.py the runtime calls of pyramid.o.
 
-  * CPU: the pyramid kernels are sm_90a and each has a DISPATCH row; the level rule; the restatement equals the
-    compiled reference CLI (when oracle/_ref is built) on lena and on template / scene pairs of different sizes, one
-    of which the stale buffer changes.
+  * CPU: the level rule; the restatement equals the compiled reference CLI (when oracle/_ref is built) on lena and on
+    template / scene pairs of different sizes, one of which the stale buffer changes.
   * GPU: every frame bit-exact against the restatement -- keypoints up to the count, untouched slots after it, every
     pyramid byte and every score-map byte with the caller's bytes as the maps' start -- at tiled and generic widths,
     L = 1..4 and a request for 5, skipped early levels, corner-rich frames whose last level's per-frame cap truncates,
@@ -37,11 +36,6 @@ QUOTA, MERGE = "gsb::k_pyr_quota", "gsb::k_pyr_merge"
 FAST_T, FAST_G = "gsb::k_fast_tiled2<true>", "gsb::k_fast_tiled2<false>"   # TMA tile loads, or plain loads
 SELECT, BRIEF_W, BRIEF_B = "gsb::k_orb_select", "gsb::k_orb_brief<true>", "gsb::k_orb_brief<false>"
 DOWN = "gsb::k_downsample_vec"
-# kernel -> the cases of this file that must launch it (test ids), checked by the census below
-DISPATCH = {
-    QUOTA: ("test_pyramid_vs_restatement[*]",),
-    MERGE: ("test_pyramid_vs_restatement[*]",),
-}
 BUF = 1024 * 1024        # nanomagick.c:299
 
 
@@ -64,16 +58,6 @@ def pyramid_lib():
 
 
 # ---- CPU: the library --------------------------------------------------------------------------------------------------
-def _pyr_sass():
-    return {k: v for k, v in L.sass_functions().items() if k.startswith("gsb::k_pyr_")}
-
-
-def test_every_kernel_is_sm90a_with_a_dispatch_row():
-    sass = _pyr_sass()
-    assert sass and all(body.startswith("code for sm_90a\n") for body in sass.values())
-    assert set(sass) == set(DISPATCH), (sorted(sass), sorted(DISPATCH))
-
-
 def test_levels_follow_the_helper_rule():
     lp = pyramid_lib()
     sides = [1, 7, 31, 32, 63, 64, 65, 127, 128, 129, 255, 256, 257, 300, 640, 1080, 1920, 4096]

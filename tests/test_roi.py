@@ -2,14 +2,13 @@
 with the reference's gs_crop followed by gs_resize_nn or gs_resize.
 
 gso_crop / gso_resize_nn (tests/_libs.py) restate the reference's two calls in numpy, 32-bit wrapping arithmetic included; the
-bilinear half of the composition is the C oracle's gso_resize (tests/_libs.py).  DISPATCH is the coverage record of the
-region kernels (gsb::k_roi_*): every one of them in the library's SASS, with the cases that must launch it.
-test_host_logic.py checks the exports and the binding table, test_streams.py the runtime calls of roi.o, and
-test_dispatch_paths.py that its launches go through gsb::launch.
+bilinear half of the composition is the C oracle's gso_resize (tests/_libs.py).  test_dispatch_paths.py has the rows
+that pick each region kernel (gsb::k_roi_*) and checks that its launches go through gsb::launch; test_host_logic.py
+checks the exports, the binding table and that every kernel is sm_90a, test_streams.py the runtime calls of roi.o.
 
-  * CPU: the region kernels are sm_90a and each has a DISPATCH row; the restatement equals the reference's gs_crop /
-    gs_resize_nn (when oracle/_ref is built), wrap cases included; the host asserts abort with the reference's message
-    and an unknown mode is an error.
+  * CPU: the copy kernel's SASS moves 16-byte blocks; the restatement equals the reference's gs_crop / gs_resize_nn
+    (when oracle/_ref is built), wrap cases included; the host asserts abort with the reference's message and an
+    unknown mode is an error.
   * GPU: both entry points against the composition (host regions at TMA-friendly and ragged widths, odd offsets,
     misaligned pointers; device lists with and without counts, untouched slots past the counts, invalid regions,
     a source batch over 4 GiB); LBP detection chained into the region call on the device counts; the CLI's crop
@@ -32,12 +31,6 @@ from _gpu import O, Region, frames, lib, stream, traced, witness, witnessed  # n
 ROOT = L.ROOT
 NEAREST, BILINEAR = 0, 1
 COPY, NN, BL = "gsb::k_roi_copy", "gsb::k_roi_gather<0>", "gsb::k_roi_gather<1>"
-# kernel -> the cases of this file that must launch it (test ids), checked by the census below
-DISPATCH = {
-    COPY: ("test_crop_resize_vs_oracle[crop-*]", "test_rois_resize_vs_oracle[*]"),
-    NN: ("test_crop_resize_vs_oracle[nn-*]", "test_rois_resize_vs_oracle[nearest-*]"),
-    BL: ("test_crop_resize_vs_oracle[bl-*]", "test_rois_resize_vs_oracle[bilinear-*]"),
-}
 
 
 def roi_lib():
@@ -46,16 +39,10 @@ def roi_lib():
 
 
 # ---- CPU: the library --------------------------------------------------------------------------------------------------
-def _roi_sass():
-    return {k: v for k, v in L.sass_functions().items() if k.startswith("gsb::k_roi_")}
-
-
-def test_every_kernel_is_sm90a_with_a_dispatch_row():
-    sass = _roi_sass()
-    assert sass and all(body.startswith("code for sm_90a\n") for body in sass.values())
-    assert set(sass) == set(DISPATCH), (sorted(sass), sorted(DISPATCH))
-    # the copy kernel moves aligned 16-byte blocks (funnel-shifted into place) and stores 16-byte chunks
-    assert "LDG.E.128.CONSTANT" in sass[COPY] and "STG.E.EF.128" in sass[COPY] and "SHF.R" in sass[COPY]
+def test_copy_kernel_moves_16_byte_blocks():
+    """the copy kernel loads aligned 16-byte blocks, funnel-shifts them into place and stores 16-byte chunks"""
+    sass = L.sass_functions()[COPY]
+    assert "LDG.E.128.CONSTANT" in sass and "STG.E.EF.128" in sass and "SHF.R" in sass
 
 
 # ---- CPU: the restatement against the reference ------------------------------------------------------------------------
