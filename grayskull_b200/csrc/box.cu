@@ -285,11 +285,13 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 
 // ---- fused gs_blur(r) -> gs_sobel: the blurred frame never goes to HBM ------------------------
 // gs_b200_blur_sobel_batch(dst, src, r) == gs_blur(tmp, src, r); gs_sobel(dst, tmp) bit for bit (dst's 1-px
-// frame untouched, like gs_sobel), with 1 B/px read + 1 B/px written instead of 4 B/px.  A CTA makes 240 sobel
-// columns x BS_TH rows in two phases with one barrier between them:
-//   A. blur on the tensor cores.  One TMA box loads input bytes [xb, xb + 272) x rows [Y - 8, Y + BS_BROWS + 8),
-//      Y = the tile's first blurred row; outside the image reads as 0, a clipped tap's contribution to the sum.  A
-//      warp walks 16-column strips (blurred columns [c0, c0 + 16), c0 = xb + 8 + 16 s) down the tile:
+// frame untouched, like gs_sobel), with 1 B/px read + 1 B/px written instead of 4 B/px.  A CTA makes 256 sobel
+// columns [x0, x0 + 256) x BS_TH rows in two phases with one barrier between them:
+//   A. blur on the tensor cores.  One TMA box loads input bytes [xb, xb + 304), xb = x0 - 16, x rows [Y - 8,
+//      Y + BS_BROWS + 8), Y = the tile's first blurred row; outside the image reads as 0, a clipped tap's contribution
+//      to the sum.  17 16-column strips (blurred columns [c0, c0 + 16), c0 = xb + 8 + 16 s) cover the blurred columns
+//      [x0 - 1, x0 + 256] that the sobel reads.  Warp w walks strips w and w + 8 down the tile, and warps 0..6 make
+//      one 16-row step each of strip 16, so that no warp holds up the barrier by more than that one step:
 //      1. horizontal sums, transposed: H^T = Bh * img with mma.m16n8k32.u8 (A = the constant 0/1 band, 16 output
 //         columns x 32 input columns [c0 - 8, c0 + 24), enough for R <= 8; B = 8 image rows, one LDS.32 per register:
 //         a thread's 4 bytes are consecutive bytes of one row).  H <= 15 * 255 = 3825;
@@ -305,25 +307,29 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 //         window anywhere takes each pixel's (inv, k) from the 226-entry table;
 //      5. two quotients of a row are adjacent columns of the MMA's D fragment: one IMAD packs their low bytes, one
 //         STS.U16 stores them to the blurred tile.
-//   B. sobel from the blurred tile, as k_stencil3_tma: each warp walks a 16-row band, each lane 8 columns, with the
-//      previous two rows' partials in registers (pairs.cuh).  The lanes holding column 0 or w-1 keep dst's byte
-//      there by writing the other seven bytes as three stores, so the kernel never reads dst.
+//   B. sobel from the blurred tile, as k_stencil3_tma: warps 0..6 walk a 16-row band each (the last one 14 rows),
+//      each lane 8 columns, with the previous two rows' partials in registers (pairs.cuh).  All 32 lanes are live, so
+//      a warp row stores 256 bytes in whole 32-byte sectors.  The lanes holding column 0 or w-1 keep dst's byte there
+//      by writing the other seven bytes as three stores, so the kernel never reads dst.
 // Blurred pixels outside the image (garbage counts, quotients possibly > 255) come in whole rows or in column pairs
 // (2j, 2j+1) that the packing keeps together, and feed only sobel outputs that are never written.
-constexpr int BS_STRIDE = 240;                 // sobel columns per tile (lanes 0..29 x 8 pixels)
-constexpr int BS_PW = 68;                      // tile pitch in words: 68 = 4 mod 32, conflict-free MMA operand loads
-constexpr int BS_STEPS = 8;                    // 16-row blur steps per tile
+constexpr int BS_STRIDE = 256;                 // sobel columns per tile (32 lanes x 8 pixels)
+constexpr int BS_IN_PW = 76;                   // input tile pitch in words: 76 = 12 mod 32, conflict-free MMA B loads
+constexpr int BS_BL_PW = 68;                   // blurred tile pitch in words: 17 strips of 16 bytes
+constexpr int BS_STEPS = 7;                    // 16-row blur steps per tile
 constexpr int BS_WARPS = 8;
 constexpr int BS_THREADS = BS_WARPS * 32;
 constexpr int BS_BROWS = 16 * BS_STEPS;        // blurred rows per tile
 constexpr int BS_TH = BS_BROWS - 2;            // sobel rows per tile
 constexpr int BS_IN_ROWS = BS_BROWS + 16;      // input rows: 8 above and below the blurred rows
-constexpr int BS_STRIPS = 16;                  // 16-column blur strips: blurred columns [xb + 8, xb + 264)
-constexpr int BS_IN_BYTES = BS_PW * 4 * BS_IN_ROWS;
-constexpr int BS_BL_BYTES = BS_PW * 4 * BS_BROWS;
+constexpr int BS_STRIPS = 17;                  // 16-column blur strips: blurred columns [xb + 8, xb + 280)
+constexpr int BS_IN_BYTES = BS_IN_PW * 4 * BS_IN_ROWS;
+constexpr int BS_BL_BYTES = BS_BL_PW * 4 * BS_BROWS;
 constexpr int BS_SMEM = BS_IN_BYTES + BS_BL_BYTES + 226 * 8 + 16;
 static_assert(BS_IN_BYTES % 128 == 0, "the blurred tile follows the TMA destination");
-static_assert(BS_TH % 16 == 14, "phase B: the last warp's band is 14 rows");
+static_assert(BS_TH % 16 == 14 && BS_TH <= 16 * (BS_WARPS - 1), "phase B: warps 0..6, the last one's band 14 rows");
+static_assert(BS_STRIPS == 2 * BS_WARPS + 1 && BS_STEPS <= BS_WARPS, "phase A: strip 16 is one step per warp");
+static_assert(3 * (BS_SMEM + 1024) <= 233472, "three CTAs per SM (228 KB, 1 KB reserved per CTA)");
 
 // div_magic of every count 1..225 as a compile-time table: a tile with clipped windows copies it to shared memory
 // (the integer division of div_magic would put I2F / MUFU work in the kernel's prologue)
@@ -382,7 +388,7 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
   constexpr float FINV = (float)FM * 5.9604644775390625e-08f, FK = 8388608.0f - 0.5f * (float)FM;   // div_magic
 
   const unsigned frame = blockIdx.z;
-  const int xb = (int)blockIdx.x * BS_STRIDE - 16;   // image column of tile byte 0 (16-B aligned)
+  const int xb = (int)blockIdx.x * BS_STRIDE - 16;   // image column of input tile byte 0 (16-B aligned)
   const int y0 = (int)(blockIdx.y + ty0) * BS_TH;    // first sobel row of the tile
   const int Y = y0 - 1;                              // first blurred row
   if (threadIdx.x == 0) {
@@ -400,20 +406,19 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;             // MMA fragment coordinates
   // the constant A operands: ah = horizontal band (row = output column c, k = input column c0 - 8 + k), av = vertical
-  // band (row = blurred row y of the step, k = H row slot; slot 4t'+i of a pair holds tile i>>1, row 2t' + (i&1))
+  // band (row = blurred row y of the step, k = H row slot; slot k = 16 p + 4t' + i of pairs p, p + 1 holds H row
+  // 16 p + 8 (i >> 1) + 2t' + (i & 1), relative to y - 8).  An entry is 1 where |k' - 8 - row| <= R, k' = k for ah and
+  // the slot's H row for av: bit k' of the window mask M = (2^(2R+1) - 1) << (row + 8 - R), row + 8 + R <= 30.  The
+  // four bytes of register j are bits kb + i (ah) and kb + {0, 1, 8, 9} (av) of M, kb = 16 (j >> 1) + 4t resp. + 2t; a
+  // nibble spreads to the low bits of four bytes by * 0x204081 (bit i lands on 8i, and no two terms share a bit).
+  // (Testing the window per entry costs each warp about 180 instructions, some 9 % of a tile's issued work.)
   uint32_t ah[4], av[4];
 #pragma unroll
   for (int j = 0; j < 4; j++) {
-    const int row = g + 8 * (j & 1), kb = 16 * (j >> 1) + 4 * t;
-    uint32_t a = 0, v = 0;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int k = kb + i;
-      const int hrow = (k >> 4) * 16 + ((k >> 1) & 1) * 8 + 2 * ((k >> 2) & 3) + (k & 1);   // relative to y - 8
-      a |= (uint32_t)(abs(k - 8 - row) <= R) << (8 * i);
-      v |= (uint32_t)(abs(hrow - 8 - row) <= R) << (8 * i);
-    }
-    ah[j] = a, av[j] = v;
+    const uint32_t m = ((1u << (2 * R + 1)) - 1u) << (g + 8 * (j & 1) + 8 - R);
+    const uint32_t mh = m >> (16 * (j >> 1) + 4 * t), mv = m >> (16 * (j >> 1) + 2 * t);
+    ah[j] = (mh & 0xFu) * 0x204081u & 0x01010101u;
+    av[j] = ((mv & 0x3u) | (mv >> 6 & 0xCu)) * 0x204081u & 0x01010101u;
   }
 
   // built once per thread (the compiler would rebuild them per strip)
@@ -426,12 +431,13 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
 
   mbar_wait(&bar, 0);
 
-  // ---- phase A: blurred tile
-  for (int s = warp; s < BS_STRIPS; s += BS_WARPS) {
+  // ---- phase A: blurred tile.  strip(s, u0, NSTEPS) makes blurred rows [16 u0, 16 (u0 + NSTEPS)) of strip s
+  auto strip = [&](int s, int u0, auto steps_tag) {
+    constexpr int NSTEPS = decltype(steps_tag)::value;
     const int c0 = xb + 8 + 16 * s;                  // image column of the strip's first blurred column
-    if (c0 >= (int)w) break;                         // warp-uniform
-    const uint32_t *ip = in + g * BS_PW + 4 * s + t;
-    unsigned char *bp = bl + g * (BS_PW * 4) + 16 * s + 2 * t;
+    if (c0 >= (int)w || Y + 16 * u0 >= (int)h) return;   // warp-uniform
+    const uint32_t *ip = in + g * BS_IN_PW + 4 * s + t;
+    unsigned char *bp = bl + g * (BS_BL_PW * 4) + 16 * s + 2 * t;
     const bool cols_full = c0 - R >= 0 && c0 + 15 + R <= (int)w - 1;
     // clipped column counts of the thread's four columns c0 + 8 hh + 2t + e
     int cw[4];
@@ -443,7 +449,7 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
     // lo / hi operands of a pair of 8-row H tiles (input rows 16 p .. 16 p + 15), both column halves
     auto make_pair = [&](int p, uint32_t (&o)[4]) {
       uint32_t P[4], Q[4];
-      const uint32_t *r0 = ip + 16 * p * BS_PW, *r1 = r0 + 8 * BS_PW;
+      const uint32_t *r0 = ip + 16 * p * BS_IN_PW, *r1 = r0 + 8 * BS_IN_PW;
       mma_u8(P, ah, r0[0], r0[4], 0u);
       mma_u8(Q, ah, r1[0], r1[4], 0u);
 #pragma unroll
@@ -456,12 +462,12 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
     // pairs u and u+1 in registers pa / pb: pair u + 1 overwrites pair u - 1, so the MMA's B operand is (pa, pb) at
     // every step, and odd steps take the band with its two k halves swapped (slots 0..15 = pair u + 1)
     uint32_t pa[4], pb[4];
-    make_pair(0, pa);
+    make_pair(u0, pa);
     auto walk = [&](auto full_tag) {
       constexpr bool FULLW = decltype(full_tag)::value;
 #pragma unroll
-      for (int u = 0; u < BS_STEPS; u++) {
-        const int yu = Y + 16 * u;
+      for (int i = 0; i < NSTEPS; i++) {
+        const int u = u0 + i, yu = Y + 16 * u;
         if (yu >= (int)h) break;                     // warp-uniform: blurred rows below the image are never used
         make_pair(u + 1, pb);
         int ch[2] = {FULL, FULL};
@@ -487,9 +493,9 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
             }
             q[j] = __float_as_uint(__fmaf_rd(__uint_as_float(imad256(dh[j], dl[j])), inv, k));
           }
-          unsigned char *o = bp + 16 * u * (BS_PW * 4) + 8 * hh;
+          unsigned char *o = bp + 16 * u * (BS_BL_PW * 4) + 8 * hh;
           *reinterpret_cast<uint16_t *>(o) = (uint16_t)imad256(q[1], q[0]);
-          *reinterpret_cast<uint16_t *>(o + 8 * (BS_PW * 4)) = (uint16_t)imad256(q[3], q[2]);
+          *reinterpret_cast<uint16_t *>(o + 8 * (BS_BL_PW * 4)) = (uint16_t)imad256(q[3], q[2]);
         }
 #pragma unroll
         for (int j = 0; j < 4; j++) pa[j] = pb[j];
@@ -498,21 +504,26 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
     // windows clipped anywhere in the strip: per-pixel counts from the table
     if (cols_full && rows_full) walk(std::true_type{});
     else walk(std::false_type{});
-  }
+  };
+  // strips 0..15 whole, two per warp; strip 16 one step per warp, on warps 0..BS_STEPS-1 (strip 16 whole on warp 7
+  // would hold the barrier for that warp's 3 BS_STEPS steps)
+  for (int s = warp; s < 2 * BS_WARPS; s += BS_WARPS) strip(s, 0, std::integral_constant<int, BS_STEPS>{});
+  if (warp < BS_STEPS) strip(2 * BS_WARPS, warp, std::integral_constant<int, 1>{});
   __syncthreads();
 
   // ---- phase B: sobel rows y0 + 16 warp .. + nb - 1 from blurred rows one above to one below
   const int r0 = 16 * warp, nb = min(16, BS_TH - r0);
+  if (nb <= 0) return;                               // warp 7: the tile's rows are warps 0..6's bands
   const int x = xb + 16 + 8 * lane;
   const int yb = y0 + r0;
-  const bool live = lane < 30 && x < (int)w;
+  const bool live = x < (int)w;
   const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
   // a warp with a lane on column 0 or w-1 walks its own copy, so that the others keep the single 64-bit store
   const bool edge_warp = __any_sync(0xFFFFFFFFu, live && (edge_l || edge_r));
   if (!live || yb > (int)h - 2) return;
-  const uint32_t *base = reinterpret_cast<const uint32_t *>(bl) + r0 * BS_PW + 2 * lane + 1;   // blurred bytes x-4 ..
+  const uint32_t *base = reinterpret_cast<const uint32_t *>(bl) + r0 * BS_BL_PW + 2 * lane + 1;   // blurred bytes x-4 ..
   auto load_row = [&](int r) -> SobelRow {
-    const uint32_t *p = base + r * BS_PW;
+    const uint32_t *p = base + r * BS_BL_PW;
     const uint2 wm = *reinterpret_cast<const uint2 *>(p + 1);
     return sobel_row(split_pairs(p[0], wm.x, wm.y, p[3]));
   };
@@ -1168,7 +1179,7 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
     });
   CUtensorMap tmap;
   if (radius >= 1 && radius <= gsb::BX_RMAX && gsb::tma_ok(src, w) && gsb::tma_ok(dst, w) &&
-      gsb::make_tmap_u8frames(&tmap, src, w, h, n, gsb::BS_PW, gsb::BS_IN_ROWS)) {
+      gsb::make_tmap_u8frames(&tmap, src, w, h, n, gsb::BS_IN_PW, gsb::BS_IN_ROWS)) {
     static decltype(&gsb::k_blur_sobel_tma<1>) const blur_sobel_fn[gsb::BX_RMAX] = {
         gsb::k_blur_sobel_tma<1>, gsb::k_blur_sobel_tma<2>, gsb::k_blur_sobel_tma<3>, gsb::k_blur_sobel_tma<4>,
         gsb::k_blur_sobel_tma<5>, gsb::k_blur_sobel_tma<6>, gsb::k_blur_sobel_tma<7>};
