@@ -30,6 +30,7 @@
 #include <limits.h>
 #include <string.h>
 
+#include <atomic>
 #include <type_traits>
 
 #include "common.cuh"
@@ -285,8 +286,15 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 
 // ---- fused gs_blur(r) -> gs_sobel: the blurred frame never goes to HBM ------------------------
 // gs_b200_blur_sobel_batch(dst, src, r) == gs_blur(tmp, src, r); gs_sobel(dst, tmp) bit for bit (dst's 1-px
-// frame untouched, like gs_sobel), with 1 B/px read + 1 B/px written instead of 4 B/px.  A CTA makes 256 sobel
-// columns [x0, x0 + 256) x BS_TH rows in two phases with one barrier between them:
+// frame untouched, like gs_sobel), with 1 B/px read + 1 B/px written instead of 4 B/px.  The grid is the CTAs that
+// fit on the device at once (3 per SM).  Tiles are numbered in raster order (column tile fastest, then tile row, then
+// frame); CTA b starts with tile b and takes each next tile from a counter, as the hardware hands out the CTAs of a
+// grid, so the tiles in flight at any moment stay one contiguous window whose neighbours read their shared halo rows
+// and whole image rows at about the same time.  (A fixed stride of the grid's size lets the CTAs drift apart over the
+// batch and was measured 60 % slower.)  A CTA sets up once (the mbarrier, the bands of phase A, the clipped-count
+// table) and then makes each tile, 256 sobel columns [x0, x0 + 256) x BS_TH rows, in two phases with a barrier after
+// each.  The next tile's TMA box is issued into the input buffer as soon as phase A has consumed it, so it lands
+// during phase B; the k-th tile of a CTA waits for mbarrier parity k & 1.
 //   A. blur on the tensor cores.  One TMA box loads input bytes [xb, xb + 304), xb = x0 - 16, x rows [Y - 8,
 //      Y + BS_BROWS + 8), Y = the tile's first blurred row; outside the image reads as 0, a clipped tap's contribution
 //      to the sum.  17 16-column strips (blurred columns [c0, c0 + 16), c0 = xb + 8 + 16 s) cover the blurred columns
@@ -325,7 +333,7 @@ constexpr int BS_IN_ROWS = BS_BROWS + 16;      // input rows: 8 above and below 
 constexpr int BS_STRIPS = 17;                  // 16-column blur strips: blurred columns [xb + 8, xb + 280)
 constexpr int BS_IN_BYTES = BS_IN_PW * 4 * BS_IN_ROWS;
 constexpr int BS_BL_BYTES = BS_BL_PW * 4 * BS_BROWS;
-constexpr int BS_SMEM = BS_IN_BYTES + BS_BL_BYTES + 226 * 8 + 16;
+constexpr int BS_SMEM = BS_IN_BYTES + BS_BL_BYTES + 226 * 8 + 16;   // + the mbarrier and the next tile's index
 static_assert(BS_IN_BYTES % 128 == 0, "the blurred tile follows the TMA destination");
 static_assert(BS_TH % 16 == 14 && BS_TH <= 16 * (BS_WARPS - 1), "phase B: warps 0..6, the last one's band 14 rows");
 static_assert(BS_STRIPS == 2 * BS_WARPS + 1 && BS_STEPS <= BS_WARPS, "phase A: strip 16 is one step per warp");
@@ -374,33 +382,54 @@ __device__ __forceinline__ void st_cs_7of8(uint8_t *p, uint2 v, bool left) {
   }
 }
 
+// floor(x / d) for x < 2^31 by one 64-bit multiply (an integer divide would convert to float): m = ceil(2^(32 + l) / d),
+// l = ceil(log2 d), so x m / 2^(32 + l) = x / d + x (m d - 2^(32 + l)) / (d 2^(32 + l)), where the excess is below
+// 2^-(l + 1) <= 1/(2d) and the fraction of x / d at most 1 - 1/d
+struct DivBy {
+  unsigned long long m;
+  unsigned shift;
+};
+inline DivBy div_by(unsigned d) {
+  unsigned l = 0;
+  while ((1ull << l) < d) l++;
+  return DivBy{((1ull << (32 + l)) + d - 1) / d, 32 + l};
+}
+__device__ __forceinline__ unsigned div_by(unsigned x, DivBy q) { return (unsigned)((unsigned long long)x * q.m >> q.shift); }
+
 template <int R>
 __global__ void __launch_bounds__(BS_THREADS, 3)
 k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, unsigned w, unsigned h,
-                 unsigned ty0 /* first row tile of the launch: for_row_groups */) {
+                 unsigned tiles_x, unsigned tiles_y, DivBy by_x, DivBy by_y, unsigned tiles /* < 2^31 */,
+                 unsigned *__restrict__ taken /* tiles handed out past the first gridDim.x; 0 at launch */) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const uint32_t *in = reinterpret_cast<const uint32_t *>(smem_raw);          // input row i = image row Y - 8 + i
   unsigned char *bl = smem_raw + BS_IN_BYTES;                                 // blurred row i = image row Y + i
   float2 *magic = reinterpret_cast<float2 *>(smem_raw + BS_IN_BYTES + BS_BL_BYTES);
   uint64_t &bar = *reinterpret_cast<uint64_t *>(smem_raw + BS_IN_BYTES + BS_BL_BYTES + 226 * 8);
+  unsigned &next = *reinterpret_cast<unsigned *>(smem_raw + BS_IN_BYTES + BS_BL_BYTES + 226 * 8 + 8);
   constexpr int FULL = 2 * R + 1;
   constexpr unsigned FM = (16777216u + FULL * FULL - 1u) / (FULL * FULL);
   constexpr float FINV = (float)FM * 5.9604644775390625e-08f, FK = 8388608.0f - 0.5f * (float)FM;   // div_magic
 
-  const unsigned frame = blockIdx.z;
-  const int xb = (int)blockIdx.x * BS_STRIDE - 16;   // image column of input tile byte 0 (16-B aligned)
-  const int y0 = (int)(blockIdx.y + ty0) * BS_TH;    // first sobel row of the tile
-  const int Y = y0 - 1;                              // first blurred row
+  // tile index (raster order) -> column tile, tile row, frame
+  auto coords = [&](unsigned i, unsigned &x, unsigned &y, unsigned &f) {
+    y = div_by(i, by_x), f = div_by(y, by_y), x = i - y * tiles_x;
+    y -= f * tiles_y;
+  };
+  auto tma_tile = [&](unsigned i) {                  // thread 0: the input box of tile i
+    unsigned x, y, f;
+    coords(i, x, y, f);
+    mbar_expect_tx(&bar, BS_IN_BYTES);
+    tma_load_3d(smem_raw, &tmap, ((int)(x * BS_STRIDE) - 16) / 4, (int)(y * BS_TH) - 9, (int)f, &bar);
+  };
+  unsigned tile = blockIdx.x;                        // the grid is at most `tiles` CTAs
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
     mbar_fence_init();
-    mbar_expect_tx(&bar, BS_IN_BYTES);
-    tma_load_3d(smem_raw, &tmap, xb / 4, Y - 8, frame, &bar);
+    tma_tile(tile);
   }
-  // the clipped-count division table, only in tiles with a clipped blurred pixel; built while the tile is in flight
-  if (Y - R < 0 || Y + BS_BROWS - 1 + R > (int)h - 1 || xb + 8 - R < 0 || xb + 8 + 16 * BS_STRIPS - 1 + R > (int)w - 1) {
-    for (unsigned c = threadIdx.x + 1; c < 226; c += BS_THREADS) magic[c] = c_div_magic.e[c];
-  }
+  // the clipped-count division table, built while the first tile is in flight
+  for (unsigned c = threadIdx.x + 1; c < 226; c += BS_THREADS) magic[c] = c_div_magic.e[c];
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -427,146 +456,194 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
   // interior division constants, in registers (FFMA takes one immediate)
   float finv = FINV, fk = FK;
   asm("" : "+f"(finv), "+f"(fk));
-  const bool rows_full = Y - R >= 0 && Y + BS_BROWS - 1 + R <= (int)h - 1;
 
-  mbar_wait(&bar, 0);
+  // Every thread runs every tile to both of its barriers: the work a warp or a lane has no part in is skipped, never
+  // left by a return.  The last tile issues no load, so no TMA is in flight when the CTA exits.
+#pragma unroll 1
+  for (unsigned it = 0; tile < tiles; it++) {
+    // the CTA's next tile: the next index not yet handed out, taken now and used after phase A (the atomic's latency
+    // hides behind it)
+    unsigned ticket = 0;
+    if (threadIdx.x == 0) ticket = gridDim.x + atomicAdd(taken, 1u);
+    unsigned tx, ty, frame;
+    coords(tile, tx, ty, frame);
+    const int xb = (int)(tx * BS_STRIDE) - 16;         // image column of input tile byte 0 (16-B aligned)
+    const int y0 = (int)(ty * BS_TH);                  // first sobel row of the tile
+    const int Y = y0 - 1;                              // first blurred row
+    const bool rows_full = Y - R >= 0 && Y + BS_BROWS - 1 + R <= (int)h - 1;
 
-  // ---- phase A: blurred tile.  strip(s, u0, NSTEPS) makes blurred rows [16 u0, 16 (u0 + NSTEPS)) of strip s
-  auto strip = [&](int s, int u0, auto steps_tag) {
-    constexpr int NSTEPS = decltype(steps_tag)::value;
-    const int c0 = xb + 8 + 16 * s;                  // image column of the strip's first blurred column
-    if (c0 >= (int)w || Y + 16 * u0 >= (int)h) return;   // warp-uniform
-    const uint32_t *ip = in + g * BS_IN_PW + 4 * s + t;
-    unsigned char *bp = bl + g * (BS_BL_PW * 4) + 16 * s + 2 * t;
-    const bool cols_full = c0 - R >= 0 && c0 + 15 + R <= (int)w - 1;
-    // clipped column counts of the thread's four columns c0 + 8 hh + 2t + e
-    int cw[4];
+    mbar_wait(&bar, it & 1);
+
+    // ---- phase A: blurred tile.  strip(s, u0, NSTEPS) makes blurred rows [16 u0, 16 (u0 + NSTEPS)) of strip s
+    auto strip = [&](int s, int u0, auto steps_tag) {
+      constexpr int NSTEPS = decltype(steps_tag)::value;
+      const int c0 = xb + 8 + 16 * s;                  // image column of the strip's first blurred column
+      if (c0 >= (int)w || Y + 16 * u0 >= (int)h) return;   // warp-uniform
+      const uint32_t *ip = in + g * BS_IN_PW + 4 * s + t;
+      unsigned char *bp = bl + g * (BS_BL_PW * 4) + 16 * s + 2 * t;
+      const bool cols_full = c0 - R >= 0 && c0 + 15 + R <= (int)w - 1;
+      // clipped column counts of the thread's four columns c0 + 8 hh + 2t + e
+      int cw[4];
 #pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int c = c0 + 8 * (j >> 1) + 2 * t + (j & 1);
-      cw[j] = max(min(c + R, (int)w - 1) - max(c - R, 0) + 1, 1);
-    }
-    // lo / hi operands of a pair of 8-row H tiles (input rows 16 p .. 16 p + 15), both column halves
-    auto make_pair = [&](int p, uint32_t (&o)[4]) {
-      uint32_t P[4], Q[4];
-      const uint32_t *r0 = ip + 16 * p * BS_IN_PW, *r1 = r0 + 8 * BS_IN_PW;
-      mma_u8(P, ah, r0[0], r0[4], 0u);
-      mma_u8(Q, ah, r1[0], r1[4], 0u);
-#pragma unroll
-      for (int hh = 0; hh < 2; hh++) {
-        const uint32_t x = prmt(P[2 * hh], P[2 * hh + 1], 0x5140), y = prmt(Q[2 * hh], Q[2 * hh + 1], 0x5140);
-        o[2 * hh] = prmt(x, y, 0x5410);        // lo bytes
-        o[2 * hh + 1] = prmt(x, y, 0x7632);    // hi bytes
+      for (int j = 0; j < 4; j++) {
+        const int c = c0 + 8 * (j >> 1) + 2 * t + (j & 1);
+        cw[j] = max(min(c + R, (int)w - 1) - max(c - R, 0) + 1, 1);
       }
-    };
-    // pairs u and u+1 in registers pa / pb: pair u + 1 overwrites pair u - 1, so the MMA's B operand is (pa, pb) at
-    // every step, and odd steps take the band with its two k halves swapped (slots 0..15 = pair u + 1)
-    uint32_t pa[4], pb[4];
-    make_pair(u0, pa);
-    auto walk = [&](auto full_tag) {
-      constexpr bool FULLW = decltype(full_tag)::value;
-#pragma unroll
-      for (int i = 0; i < NSTEPS; i++) {
-        const int u = u0 + i, yu = Y + 16 * u;
-        if (yu >= (int)h) break;                     // warp-uniform: blurred rows below the image are never used
-        make_pair(u + 1, pb);
-        int ch[2] = {FULL, FULL};
-        if (!FULLW) {
-#pragma unroll
-          for (int e = 0; e < 2; e++) {
-            const int y = yu + g + 8 * e;
-            ch[e] = max(min(y + R, (int)h - 1) - max(y - R, 0) + 1, 1);
-          }
-        }
+      // lo / hi operands of a pair of 8-row H tiles (input rows 16 p .. 16 p + 15), both column halves
+      auto make_pair = [&](int p, uint32_t (&o)[4]) {
+        uint32_t P[4], Q[4];
+        const uint32_t *r0 = ip + 16 * p * BS_IN_PW, *r1 = r0 + 8 * BS_IN_PW;
+        mma_u8(P, ah, r0[0], r0[4], 0u);
+        mma_u8(Q, ah, r1[0], r1[4], 0u);
 #pragma unroll
         for (int hh = 0; hh < 2; hh++) {
-          uint32_t dl[4], dh[4];
-          mma_u8(dl, av, pa[2 * hh], pb[2 * hh], 0x4B000000u);
-          mma_u8(dh, av, pa[2 * hh + 1], pb[2 * hh + 1], 0u);
-          uint32_t q[4];
-#pragma unroll
-          for (int j = 0; j < 4; j++) {             // D element j: row g + 8 (j >> 1), column 8 hh + 2t + (j & 1)
-            float inv = finv, k = fk;
-            if (!FULLW) {
-              const float2 m = magic[cw[2 * hh + (j & 1)] * ch[j >> 1]];
-              inv = m.x, k = m.y;
-            }
-            q[j] = __float_as_uint(__fmaf_rd(__uint_as_float(imad256(dh[j], dl[j])), inv, k));
-          }
-          unsigned char *o = bp + 16 * u * (BS_BL_PW * 4) + 8 * hh;
-          *reinterpret_cast<uint16_t *>(o) = (uint16_t)imad256(q[1], q[0]);
-          *reinterpret_cast<uint16_t *>(o + 8 * (BS_BL_PW * 4)) = (uint16_t)imad256(q[3], q[2]);
+          const uint32_t x = prmt(P[2 * hh], P[2 * hh + 1], 0x5140), y = prmt(Q[2 * hh], Q[2 * hh + 1], 0x5140);
+          o[2 * hh] = prmt(x, y, 0x5410);        // lo bytes
+          o[2 * hh + 1] = prmt(x, y, 0x7632);    // hi bytes
         }
+      };
+      // pairs u and u+1 in registers pa / pb: pair u + 1 overwrites pair u - 1, so the MMA's B operand is (pa, pb) at
+      // every step, and odd steps take the band with its two k halves swapped (slots 0..15 = pair u + 1)
+      uint32_t pa[4], pb[4];
+      make_pair(u0, pa);
+      auto walk = [&](auto full_tag) {
+        constexpr bool FULLW = decltype(full_tag)::value;
 #pragma unroll
-        for (int j = 0; j < 4; j++) pa[j] = pb[j];
-      }
+        for (int i = 0; i < NSTEPS; i++) {
+          const int u = u0 + i, yu = Y + 16 * u;
+          if (yu >= (int)h) break;                     // warp-uniform: blurred rows below the image are never used
+          make_pair(u + 1, pb);
+          int ch[2] = {FULL, FULL};
+          if (!FULLW) {
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+              const int y = yu + g + 8 * e;
+              ch[e] = max(min(y + R, (int)h - 1) - max(y - R, 0) + 1, 1);
+            }
+          }
+#pragma unroll
+          for (int hh = 0; hh < 2; hh++) {
+            uint32_t dl[4], dh[4];
+            mma_u8(dl, av, pa[2 * hh], pb[2 * hh], 0x4B000000u);
+            mma_u8(dh, av, pa[2 * hh + 1], pb[2 * hh + 1], 0u);
+            uint32_t q[4];
+#pragma unroll
+            for (int j = 0; j < 4; j++) {             // D element j: row g + 8 (j >> 1), column 8 hh + 2t + (j & 1)
+              float inv = finv, k = fk;
+              if (!FULLW) {
+                const float2 m = magic[cw[2 * hh + (j & 1)] * ch[j >> 1]];
+                inv = m.x, k = m.y;
+              }
+              q[j] = __float_as_uint(__fmaf_rd(__uint_as_float(imad256(dh[j], dl[j])), inv, k));
+            }
+            unsigned char *o = bp + 16 * u * (BS_BL_PW * 4) + 8 * hh;
+            *reinterpret_cast<uint16_t *>(o) = (uint16_t)imad256(q[1], q[0]);
+            *reinterpret_cast<uint16_t *>(o + 8 * (BS_BL_PW * 4)) = (uint16_t)imad256(q[3], q[2]);
+          }
+#pragma unroll
+          for (int j = 0; j < 4; j++) pa[j] = pb[j];
+        }
+      };
+      // windows clipped anywhere in the strip: per-pixel counts from the table
+      if (cols_full && rows_full) walk(std::true_type{});
+      else walk(std::false_type{});
     };
-    // windows clipped anywhere in the strip: per-pixel counts from the table
-    if (cols_full && rows_full) walk(std::true_type{});
-    else walk(std::false_type{});
-  };
-  // strips 0..15 whole, two per warp; strip 16 one step per warp, on warps 0..BS_STEPS-1 (strip 16 whole on warp 7
-  // would hold the barrier for that warp's 3 BS_STEPS steps)
-  for (int s = warp; s < 2 * BS_WARPS; s += BS_WARPS) strip(s, 0, std::integral_constant<int, BS_STEPS>{});
-  if (warp < BS_STEPS) strip(2 * BS_WARPS, warp, std::integral_constant<int, 1>{});
-  __syncthreads();
+    // strips 0..15 whole, two per warp; strip 16 one step per warp, on warps 0..BS_STEPS-1 (strip 16 whole on warp 7
+    // would hold the barrier for that warp's 3 BS_STEPS steps)
+    for (int s = warp; s < 2 * BS_WARPS; s += BS_WARPS) strip(s, 0, std::integral_constant<int, BS_STEPS>{});
+    if (warp < BS_STEPS) strip(2 * BS_WARPS, warp, std::integral_constant<int, 1>{});
+    __syncthreads();
 
-  // ---- phase B: sobel rows y0 + 16 warp .. + nb - 1 from blurred rows one above to one below
-  const int r0 = 16 * warp, nb = min(16, BS_TH - r0);
-  if (nb <= 0) return;                               // warp 7: the tile's rows are warps 0..6's bands
-  const int x = xb + 16 + 8 * lane;
-  const int yb = y0 + r0;
-  const bool live = x < (int)w;
-  const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
-  // a warp with a lane on column 0 or w-1 walks its own copy, so that the others keep the single 64-bit store
-  const bool edge_warp = __any_sync(0xFFFFFFFFu, live && (edge_l || edge_r));
-  if (!live || yb > (int)h - 2) return;
-  const uint32_t *base = reinterpret_cast<const uint32_t *>(bl) + r0 * BS_BL_PW + 2 * lane + 1;   // blurred bytes x-4 ..
-  auto load_row = [&](int r) -> SobelRow {
-    const uint32_t *p = base + r * BS_BL_PW;
-    const uint2 wm = *reinterpret_cast<const uint2 *>(p + 1);
-    return sobel_row(split_pairs(p[0], wm.x, wm.y, p[3]));
-  };
-  uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
-  SobelRow ra = load_row(0), rb = load_row(1);
-  auto walk_full = [&](auto edge_tag) {
+    // the input tile is consumed: the next tile's box lands in it during this tile's sobel.  The CTA read it through
+    // the generic proxy and the TMA writes it through the async proxy, hence the proxy fence after the barrier.
+    if (threadIdx.x == 0) {
+      next = ticket;
+      if (ticket < tiles) {
+        fence_proxy_async();
+        tma_tile(ticket);
+      }
+    }
+
+    // ---- phase B: sobel rows y0 + 16 warp .. + nb - 1 from blurred rows one above to one below
+    const int r0 = 16 * warp, nb = min(16, BS_TH - r0);
+    if (nb > 0) {                                      // warp 7 has no band: the tile's rows are warps 0..6's
+      const int x = xb + 16 + 8 * lane;
+      const int yb = y0 + r0;
+      const bool live = x < (int)w;
+      const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
+      // a warp with a lane on column 0 or w-1 walks its own copy, so that the others keep the single 64-bit store
+      const bool edge_warp = __any_sync(0xFFFFFFFFu, live && (edge_l || edge_r));
+      if (live && yb <= (int)h - 2) {
+        const uint32_t *base = reinterpret_cast<const uint32_t *>(bl) + r0 * BS_BL_PW + 2 * lane + 1;   // bytes x-4 ..
+        auto load_row = [&](int r) -> SobelRow {
+          const uint32_t *p = base + r * BS_BL_PW;
+          const uint2 wm = *reinterpret_cast<const uint2 *>(p + 1);
+          return sobel_row(split_pairs(p[0], wm.x, wm.y, p[3]));
+        };
+        uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
+        SobelRow ra = load_row(0), rb = load_row(1);
+        auto walk_full = [&](auto edge_tag) {
 #pragma unroll
-    for (int i = 0; i < 16; i++) {
-      if (i >= BS_TH % 16 && i >= nb) break;
-      const SobelRow rc = load_row(i + 2);
-      const uint2 so = sobel_out(ra, rb, rc);
-      if (!decltype(edge_tag)::value) {
-        st_cs_u2(outp, so);
-      } else {                                       // predicated, no lane branches
-        if (!edge_l && !edge_r) st_cs_u2(outp, so);
-        if (edge_l) st_cs_7of8(outp, so, true);
-        if (edge_r) st_cs_7of8(outp, so, false);
-      }
-      outp += w;
-      ra = rb;
-      rb = rc;
-    }
-  };
-  if (yb >= 1 && yb + nb - 1 <= (int)h - 2) {
-    if (edge_warp) walk_full(std::true_type{});
-    else walk_full(std::false_type{});
-  } else {
+          for (int i = 0; i < 16; i++) {
+            if (i >= BS_TH % 16 && i >= nb) break;
+            const SobelRow rc = load_row(i + 2);
+            const uint2 so = sobel_out(ra, rb, rc);
+            if (!decltype(edge_tag)::value) {
+              st_cs_u2(outp, so);
+            } else {                                   // predicated, no lane branches
+              if (!edge_l && !edge_r) st_cs_u2(outp, so);
+              if (edge_l) st_cs_7of8(outp, so, true);
+              if (edge_r) st_cs_7of8(outp, so, false);
+            }
+            outp += w;
+            ra = rb;
+            rb = rc;
+          }
+        };
+        if (yb >= 1 && yb + nb - 1 <= (int)h - 2) {
+          if (edge_warp) walk_full(std::true_type{});
+          else walk_full(std::false_type{});
+        } else {
 #pragma unroll 1
-    for (int i = 0; i < nb; i++) {
-      const int y = yb + i;
-      if (y > (int)h - 2) break;
-      const SobelRow rc = load_row(i + 2);
-      if (y >= 1) {
-        const uint2 so = sobel_out(ra, rb, rc);
-        if (edge_l) st_cs_7of8(outp, so, true);
-        else if (edge_r) st_cs_7of8(outp, so, false);
-        else st_cs_u2(outp, so);
+          for (int i = 0; i < nb; i++) {
+            const int y = yb + i;
+            if (y > (int)h - 2) break;
+            const SobelRow rc = load_row(i + 2);
+            if (y >= 1) {
+              const uint2 so = sobel_out(ra, rb, rc);
+              if (edge_l) st_cs_7of8(outp, so, true);
+              else if (edge_r) st_cs_7of8(outp, so, false);
+              else st_cs_u2(outp, so);
+            }
+            outp += w;
+            ra = rb;
+            rb = rc;
+          }
+        }
       }
-      outp += w;
-      ra = rb;
-      rb = rc;
     }
+    __syncthreads();                                   // the next tile's phase A overwrites the blurred tile
+    tile = next;                                       // written before the barrier above, rewritten after the next
   }
+}
+
+// CTAs of k_blur_sobel_tma<r> (kernel k) that one SM holds at once (its launch bounds ask for 3), asked once per device
+// and radius: the kernel's grid is that many CTAs per SM
+static int blur_sobel_ctas_per_sm(unsigned r, const void *k, int *ctas) {
+  static std::atomic<int> cache[64][BX_RMAX];
+  int dev = 0;
+  GSB_CHECK(cudaGetDevice(&dev));
+  std::atomic<int> *slot = dev >= 0 && dev < 64 ? &cache[dev][r - 1] : nullptr;
+  int c = slot ? slot->load(std::memory_order_relaxed) : 0;
+  if (!c) {
+    // the query counts the dynamic shared memory against the kernel's opted-in limit
+    if (int rc = opt_in_smem(k, BS_SMEM, __FILE__, __LINE__)) return rc;
+    GSB_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, k, BS_THREADS, BS_SMEM));
+    if (c < 1) c = 1;                                  // the launch reports why none fits
+    if (slot) slot->store(c, std::memory_order_relaxed);
+  }
+  *ctas = c;
+  return 0;
 }
 
 // ---- wide radii (8 <= r <= 120): radius-independent work, u32 window sums -------------------
@@ -1171,7 +1248,7 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
   GSB_ASSERT(dst && src && w > 0 && h > 0);  // reference :269, :307
   cudaStream_t s = static_cast<cudaStream_t>(st);
   if (n == 0 || w < 3 || h < 3) return 0;    // gs_sobel writes nothing below 3x3 (reference :308-309)
-  // k_blur_sobel_tma puts the frame in grid z, and the fall-back's scratch batch stays at one group
+  // the fall-back's scratch batch stays at one group
   if (n > gsb::GRID_FRAMES)
     return gsb::for_frame_groups(n, [&](unsigned f0, unsigned c) {
       const size_t o = (size_t)f0 * w * h;
@@ -1183,11 +1260,20 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
     static decltype(&gsb::k_blur_sobel_tma<1>) const blur_sobel_fn[gsb::BX_RMAX] = {
         gsb::k_blur_sobel_tma<1>, gsb::k_blur_sobel_tma<2>, gsb::k_blur_sobel_tma<3>, gsb::k_blur_sobel_tma<4>,
         gsb::k_blur_sobel_tma<5>, gsb::k_blur_sobel_tma<6>, gsb::k_blur_sobel_tma<7>};
+    const auto k = blur_sobel_fn[radius - 1];
     const unsigned tiles_x = (w + gsb::BS_STRIDE - 1) / gsb::BS_STRIDE, tiles_y = (h + gsb::BS_TH - 1) / gsb::BS_TH;
-    return gsb::for_row_groups(tiles_y, [&](unsigned t0, unsigned c) {
-      return gsb::launch(__FILE__, __LINE__, blur_sobel_fn[radius - 1], dim3(tiles_x, c, n), gsb::BS_THREADS, gsb::BS_SMEM, s,
-                         tmap, dst, w, h, t0);
-    });
+    const unsigned long long tiles = (unsigned long long)tiles_x * tiles_y * n;
+    // tile indices are 31-bit: a frame of more than one tile holds at least 408 bytes per tile, so 2^31 tiles need 876 GB
+    if (tiles > INT_MAX) return gsb::record_error(cudaErrorInvalidValue, __FILE__, __LINE__);
+    int ctas = 0;
+    if (int rc = gsb::blur_sobel_ctas_per_sm(radius, reinterpret_cast<const void *>(k), &ctas)) return rc;
+    // resident CTAs only; each takes its next tile from a counter, so the tiles in flight stay one raster window
+    const unsigned long long resident = (unsigned long long)ctas * gsb::sm_count(), grid = tiles < resident ? tiles : resident;
+    unsigned *taken = static_cast<unsigned *>(gsb::workspace(s, gsb::WS_BLUR_SOBEL_TILES, sizeof(unsigned)));
+    if (!taken) return gsb::workspace_error();
+    GSB_CHECK(cudaMemsetAsync(taken, 0, sizeof(unsigned), s));
+    return gsb::launch(__FILE__, __LINE__, k, dim3((unsigned)grid), gsb::BS_THREADS, gsb::BS_SMEM, s, tmap, dst, w, h,
+                       tiles_x, tiles_y, gsb::div_by(tiles_x), gsb::div_by(tiles_y), (unsigned)tiles, taken);
   }
   // other radii / ragged widths: the two per-op kernels through a scratch frame batch (same result, 4 B/px)
   uint8_t *tmp = static_cast<uint8_t *>(gsb::workspace(s, gsb::WS_STAGE_FUSED, (size_t)w * h * n));

@@ -99,7 +99,9 @@ enum { WS_INTEGRAL = 0, WS_FAST_A, WS_FAST_B, WS_ORB_A, WS_ORB_B, WS_LBP_A, WS_L
        WS_STAGE_A, WS_STAGE_B, WS_STAGE_C, WS_STAGE_D, WS_HIST, WS_STAGE_FUSED, WS_BLOB_A, WS_BLOB_B, WS_BLOB_C, WS_MORPH,
        // csrc/pyramid.cu: per-level keypoint lists, the last level's FAST candidates, per-level counts.  Distinct from
        // WS_FAST_* / WS_ORB_*, which the calls it makes in between use.
-       WS_PYR_LISTS, WS_PYR_CAND, WS_PYR_COUNTS, WS_SLOTS };
+       WS_PYR_LISTS, WS_PYR_CAND, WS_PYR_COUNTS,
+       // csrc/box.cu: the tile counter of k_blur_sobel_tma
+       WS_BLUR_SOBEL_TILES, WS_SLOTS };
 
 // 3-D tensor map over n dense u8 frames of w x h, viewed as 32-bit words {w/4, h, n}
 // (TMA boxes are limited to 256 elements per dimension: u32 elements give 1 KiB wide boxes).
@@ -124,6 +126,11 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, unsigned count) {
 // make the barrier init visible to the async (TMA) proxy before the first bulk copy targets it
 __device__ __forceinline__ void mbar_fence_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+// order the generic-proxy shared-memory accesses before it (the whole CTA's, after a barrier) before later async-proxy
+// ones: a TMA load may then refill a buffer that the CTA has just read
+__device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, unsigned bytes) {

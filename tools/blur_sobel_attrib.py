@@ -6,11 +6,14 @@ Prints the card's name, power limit and SM clocks, then, each in ms and GB/s (CU
   * copy    device-to-device torch copy_ of the c2 batch (256 x 4096^2 u8): the practical HBM ceiling of a
             1:1 read:write stream, the figure the kernels below are set against;
   * sobel   gs_b200_sobel_batch at c2's shape;
-  * fused   gs_b200_blur_sobel_batch, r=5, at c2's shape and at c5's (1024 x 1920x1080).
-Every kernel moves 1 B read + 1 B written per pixel, so GB/s = 2 * pixels / time for all of them.  Several builds
-of the library (--lib, default: this tree's) are loaded side by side and timed alternately, --reps times; the
-median and the spread (max - min over the median) are reported per build.  Needs a CUDA device; writes only the
---out file.
+  * fused   gs_b200_blur_sobel_batch, r=5, at c2's shape, at c5's (1024 x 1920x1080) and on one 4096^2 frame,
+            whose 16 MB in and 16 MB out stay in the 50 MB L2 across the back-to-back calls.
+Every kernel moves 1 B read + 1 B written per pixel, so GB/s = 2 * pixels / time for all of them.  The fused rows
+also give the time per 256 x 110 tile: the L2-resident frame's against c2's tells whether the kernel waits on its
+tile loads from HBM (well below c2's) or is bound by issuing its instructions (about equal).  One frame is only about
+1.5 waves of resident CTAs, so that comparison is approximate.  Several builds of the library (--lib, default: this
+tree's) are loaded side by side and timed alternately, --reps times; the median and the spread (max - min over the
+median) are reported per build.  Needs a CUDA device; writes only the --out file.
 """
 import argparse
 import ctypes as C
@@ -22,7 +25,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 R = 5
-C2, C5 = (256, 4096, 4096), (1024, 1920, 1080)     # (frames, w, h)
+C2, C5, L2 = (256, 4096, 4096), (1024, 1920, 1080), (1, 4096, 4096)     # (frames, w, h)
+TW, TH = 256, 110                                                      # the fused kernel's tile
 
 
 def gpu_info():
@@ -66,6 +70,8 @@ def main():
 
     def timed(fn):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        # the device sleeps while the host queues the calls, so that the short L2-resident ones run back to back
+        torch.cuda._sleep(4_000_000)
         e0.record()
         for _ in range(a.iters):
             fn()
@@ -83,20 +89,22 @@ def main():
             for name, fn in fns.items():
                 ms[name].append(timed(fn))
         out = {"what": label, "frames": n, "w": w, "h": h, "builds": {}}
+        tiles = n * -(-w // TW) * -(-h // TH)
         for name, v in ms.items():
             med = statistics.median(v)
             out["builds"][name] = {"ms": v, "ms_median": med, "spread_pct": 100 * (max(v) - min(v)) / med,
-                                   "GB_s": 2 * n * w * h / med / 1e6}
+                                   "GB_s": 2 * n * w * h / med / 1e6, "us_per_tile": 1e3 * med / tiles}
         res["rows"].append(out)
         print("%-6s %4d x %dx%d  " % (label, n, w, h) +
-              "  ".join("%s %.4f ms %.0f GB/s (spread %.2f%%)" % (k, b["ms_median"], b["GB_s"], b["spread_pct"])
+              "  ".join("%s %.4f ms %.0f GB/s (spread %.2f%%)" % (k, b["ms_median"], b["GB_s"], b["spread_pct"]) +
+                        (" %.4f us/tile" % b["us_per_tile"] if label == "fused" else "")
                         for k, b in out["builds"].items()), flush=True)
         return out
 
     def check(rc):
         assert rc == 0, rc
 
-    for shape in (C2, C5):
+    for shape in (C2, C5, L2):
         n, w, h = shape
         g = torch.Generator(device="cuda").manual_seed(w * h + n)
         src = torch.randint(0, 256, (n, h, w), dtype=torch.uint8, device="cuda", generator=g)
