@@ -315,10 +315,12 @@ k_box_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ dst, u
 //         window anywhere takes each pixel's (inv, k) from the 226-entry table;
 //      5. two quotients of a row are adjacent columns of the MMA's D fragment: one IMAD packs their low bytes, one
 //         STS.U16 stores them to the blurred tile.
-//   B. sobel from the blurred tile, as k_stencil3_tma: warps 0..6 walk a 16-row band each (the last one 14 rows),
-//      each lane 8 columns, with the previous two rows' partials in registers (pairs.cuh).  All 32 lanes are live, so
-//      a warp row stores 256 bytes in whole 32-byte sectors.  The lanes holding column 0 or w-1 keep dst's byte there
-//      by writing the other seven bytes as three stores, so the kernel never reads dst.
+//   B. sobel from the blurred tile, as k_stencil3_tma: each warp walks a band of the tile's rows, 14 rows on warps 0..5
+//      and 13 on warps 6 and 7, each lane 8 columns, with the previous two rows' partials in registers (pairs.cuh).
+//      Every warp has a band because warps w and w + 4 share a scheduler (w % 4, the usual hardware assignment): with
+//      16-row bands on warps 0..6, warp 7's scheduler had half the others' phase-B work.  All 32 lanes are live, so a
+//      warp row stores 256 bytes in whole 32-byte sectors.  The lanes holding column 0 or w-1 keep dst's byte there by
+//      writing the other seven bytes as three stores, so the kernel never reads dst.
 // Blurred pixels outside the image (garbage counts, quotients possibly > 255) come in whole rows or in column pairs
 // (2j, 2j+1) that the packing keeps together, and feed only sobel outputs that are never written.
 constexpr int BS_STRIDE = 256;                 // sobel columns per tile (32 lanes x 8 pixels)
@@ -331,11 +333,12 @@ constexpr int BS_BROWS = 16 * BS_STEPS;        // blurred rows per tile
 constexpr int BS_TH = BS_BROWS - 2;            // sobel rows per tile
 constexpr int BS_IN_ROWS = BS_BROWS + 16;      // input rows: 8 above and below the blurred rows
 constexpr int BS_STRIPS = 17;                  // 16-column blur strips: blurred columns [xb + 8, xb + 280)
+constexpr int BS_BAND = (BS_TH + BS_WARPS - 1) / BS_WARPS;   // sobel rows of the longest phase-B bands: 14
+constexpr int BS_LONG = BS_TH - BS_WARPS * (BS_BAND - 1);    // warps with a band of BS_BAND rows (6); the rest, 13
 constexpr int BS_IN_BYTES = BS_IN_PW * 4 * BS_IN_ROWS;
 constexpr int BS_BL_BYTES = BS_BL_PW * 4 * BS_BROWS;
 constexpr int BS_SMEM = BS_IN_BYTES + BS_BL_BYTES + 226 * 8 + 16;   // + the mbarrier and the next tile's index
 static_assert(BS_IN_BYTES % 128 == 0, "the blurred tile follows the TMA destination");
-static_assert(BS_TH % 16 == 14 && BS_TH <= 16 * (BS_WARPS - 1), "phase B: warps 0..6, the last one's band 14 rows");
 static_assert(BS_STRIPS == 2 * BS_WARPS + 1 && BS_STEPS <= BS_WARPS, "phase A: strip 16 is one step per warp");
 static_assert(3 * (BS_SMEM + 1024) <= 233472, "three CTAs per SM (228 KB, 1 KB reserved per CTA)");
 
@@ -450,9 +453,16 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
     av[j] = ((mv & 0x3u) | (mv >> 6 & 0xCu)) * 0x204081u & 0x01010101u;
   }
 
-  // built once per thread (the compiler would rebuild them per strip)
+  // av with its two k halves swapped (A registers 0, 1 hold k 0..15 and 2, 3 hold k 16..31): the band of the steps whose
+  // B operand holds its two pairs the other way round
+  uint32_t avs[4];
+  // built once per thread (the compiler would rebuild them per strip); avs through a PRMT the compiler cannot see
+  // through, or it copies av into it before every MMA that takes it
 #pragma unroll
-  for (int j = 0; j < 4; j++) asm("" : "+r"(ah[j]), "+r"(av[j]));
+  for (int j = 0; j < 4; j++) {
+    asm("" : "+r"(ah[j]), "+r"(av[j]));
+    asm("prmt.b32 %0, %1, 0, 0x3210;" : "=r"(avs[j]) : "r"(av[j ^ 2]));
+  }
   // interior division constants, in registers (FFMA takes one immediate)
   float finv = FINV, fk = FK;
   asm("" : "+f"(finv), "+f"(fk));
@@ -503,7 +513,8 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
         }
       };
       // pairs u and u+1 in registers pa / pb: pair u + 1 overwrites pair u - 1, so the MMA's B operand is (pa, pb) at
-      // every step, and odd steps take the band with its two k halves swapped (slots 0..15 = pair u + 1)
+      // every step, and odd steps take the band with its two k halves swapped (slots 0..15 = pair u + 1).  No pair is
+      // copied from one register to another (the MMA wants its two B registers adjacent, so a copy is a MOV each)
       uint32_t pa[4], pb[4];
       make_pair(u0, pa);
       auto walk = [&](auto full_tag) {
@@ -511,8 +522,10 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
 #pragma unroll
         for (int i = 0; i < NSTEPS; i++) {
           const int u = u0 + i, yu = Y + 16 * u;
-          if (yu >= (int)h) break;                     // warp-uniform: blurred rows below the image are never used
-          make_pair(u + 1, pb);
+          // warp-uniform: blurred rows below the image are never used (a full walk has none: rows_full)
+          if (!FULLW && yu >= (int)h) break;
+          make_pair(u + 1, (i & 1) ? pa : pb);
+          const uint32_t (&band)[4] = (i & 1) ? avs : av;
           int ch[2] = {FULL, FULL};
           if (!FULLW) {
 #pragma unroll
@@ -524,8 +537,8 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
 #pragma unroll
           for (int hh = 0; hh < 2; hh++) {
             uint32_t dl[4], dh[4];
-            mma_u8(dl, av, pa[2 * hh], pb[2 * hh], 0x4B000000u);
-            mma_u8(dh, av, pa[2 * hh + 1], pb[2 * hh + 1], 0u);
+            mma_u8(dl, band, pa[2 * hh], pb[2 * hh], 0x4B000000u);
+            mma_u8(dh, band, pa[2 * hh + 1], pb[2 * hh + 1], 0u);
             uint32_t q[4];
 #pragma unroll
             for (int j = 0; j < 4; j++) {             // D element j: row g + 8 (j >> 1), column 8 hh + 2t + (j & 1)
@@ -540,8 +553,6 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
             *reinterpret_cast<uint16_t *>(o) = (uint16_t)imad256(q[1], q[0]);
             *reinterpret_cast<uint16_t *>(o + 8 * (BS_BL_PW * 4)) = (uint16_t)imad256(q[3], q[2]);
           }
-#pragma unroll
-          for (int j = 0; j < 4; j++) pa[j] = pb[j];
         }
       };
       // windows clipped anywhere in the strip: per-pixel counts from the table
@@ -564,61 +575,60 @@ k_blur_sobel_tma(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__
       }
     }
 
-    // ---- phase B: sobel rows y0 + 16 warp .. + nb - 1 from blurred rows one above to one below
-    const int r0 = 16 * warp, nb = min(16, BS_TH - r0);
-    if (nb > 0) {                                      // warp 7 has no band: the tile's rows are warps 0..6's
-      const int x = xb + 16 + 8 * lane;
-      const int yb = y0 + r0;
-      const bool live = x < (int)w;
-      const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
-      // a warp with a lane on column 0 or w-1 walks its own copy, so that the others keep the single 64-bit store
-      const bool edge_warp = __any_sync(0xFFFFFFFFu, live && (edge_l || edge_r));
-      if (live && yb <= (int)h - 2) {
-        const uint32_t *base = reinterpret_cast<const uint32_t *>(bl) + r0 * BS_BL_PW + 2 * lane + 1;   // bytes x-4 ..
-        auto load_row = [&](int r) -> SobelRow {
-          const uint32_t *p = base + r * BS_BL_PW;
-          const uint2 wm = *reinterpret_cast<const uint2 *>(p + 1);
-          return sobel_row(split_pairs(p[0], wm.x, wm.y, p[3]));
-        };
-        uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
-        SobelRow ra = load_row(0), rb = load_row(1);
-        auto walk_full = [&](auto edge_tag) {
+    // ---- phase B: sobel rows y0 + r0 .. + nb - 1 from blurred rows one above to one below.  Bands of BS_BAND rows on
+    // warps 0..BS_LONG-1 and of BS_BAND - 1 rows on the others
+    const int r0 = (BS_BAND - 1) * warp + min(warp, BS_LONG), nb = BS_BAND - (warp >= BS_LONG);
+    const int x = xb + 16 + 8 * lane;
+    const int yb = y0 + r0;
+    const bool live = x < (int)w;
+    const bool edge_l = x == 0, edge_r = x + 8 == (int)w;
+    // a warp with a lane on column 0 or w-1 walks its own copy, so that the others keep the single 64-bit store
+    const bool edge_warp = __any_sync(0xFFFFFFFFu, live && (edge_l || edge_r));
+    if (live && yb <= (int)h - 2) {
+      const uint32_t *base = reinterpret_cast<const uint32_t *>(bl) + r0 * BS_BL_PW + 2 * lane + 1;   // bytes x-4 ..
+      auto load_row = [&](int r) -> SobelRow {
+        const uint32_t *p = base + r * BS_BL_PW;
+        const uint2 wm = *reinterpret_cast<const uint2 *>(p + 1);
+        return sobel_row(split_pairs(p[0], wm.x, wm.y, p[3]));
+      };
+      uint8_t *outp = dst + (size_t)frame * w * h + (size_t)yb * w + x;
+      SobelRow ra = load_row(0), rb = load_row(1);
+      auto walk_full = [&](auto edge_tag) {
 #pragma unroll
-          for (int i = 0; i < 16; i++) {
-            if (i >= BS_TH % 16 && i >= nb) break;
-            const SobelRow rc = load_row(i + 2);
-            const uint2 so = sobel_out(ra, rb, rc);
-            if (!decltype(edge_tag)::value) {
-              st_cs_u2(outp, so);
-            } else {                                   // predicated, no lane branches
-              if (!edge_l && !edge_r) st_cs_u2(outp, so);
-              if (edge_l) st_cs_7of8(outp, so, true);
-              if (edge_r) st_cs_7of8(outp, so, false);
-            }
-            outp += w;
-            ra = rb;
-            rb = rc;
+        for (int i = 0; i < BS_BAND; i++) {
+          if (i == BS_BAND - 1 && nb < BS_BAND) break;
+          const SobelRow rc = load_row(i + 2);
+          const uint2 so = sobel_out(ra, rb, rc);
+          if (!decltype(edge_tag)::value) {
+            st_cs_u2(outp, so);
+          } else {                                     // predicated, no lane branches
+            if (!edge_l && !edge_r) st_cs_u2(outp, so);
+            if (edge_l) st_cs_7of8(outp, so, true);
+            if (edge_r) st_cs_7of8(outp, so, false);
           }
-        };
-        if (yb >= 1 && yb + nb - 1 <= (int)h - 2) {
-          if (edge_warp) walk_full(std::true_type{});
-          else walk_full(std::false_type{});
-        } else {
+          outp += w;
+          ra = rb;
+          rb = rc;
+        }
+      };
+      if (yb >= 1 && yb + nb - 1 <= (int)h - 2) {
+        if (edge_warp) walk_full(std::true_type{});
+        else walk_full(std::false_type{});
+      } else {
 #pragma unroll 1
-          for (int i = 0; i < nb; i++) {
-            const int y = yb + i;
-            if (y > (int)h - 2) break;
-            const SobelRow rc = load_row(i + 2);
-            if (y >= 1) {
-              const uint2 so = sobel_out(ra, rb, rc);
-              if (edge_l) st_cs_7of8(outp, so, true);
-              else if (edge_r) st_cs_7of8(outp, so, false);
-              else st_cs_u2(outp, so);
-            }
-            outp += w;
-            ra = rb;
-            rb = rc;
+        for (int i = 0; i < nb; i++) {
+          const int y = yb + i;
+          if (y > (int)h - 2) break;
+          const SobelRow rc = load_row(i + 2);
+          if (y >= 1) {
+            const uint2 so = sobel_out(ra, rb, rc);
+            if (edge_l) st_cs_7of8(outp, so, true);
+            else if (edge_r) st_cs_7of8(outp, so, false);
+            else st_cs_u2(outp, so);
           }
+          outp += w;
+          ra = rb;
+          rb = rc;
         }
       }
     }

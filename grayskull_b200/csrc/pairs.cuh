@@ -9,20 +9,19 @@ struct Pairs {  // pair words P_k = (x+k, x+k+2) for k = -1 .. 6, 16-bit lanes
   uint32_t m1, p0, p1, p2, p3, p4, p5, p6;
 };
 
-// wl,w0,w1,wr = image bytes [x-4,x), [x,x+4), [x+4,x+8), [x+8,x+12)
+// wl,w0,w1,wr = image bytes [x-4,x), [x,x+4), [x+4,x+8), [x+8,x+12).  Eight ALU operations: the four aligned pairs are
+// masked or permuted against zero, and each misaligned pair is one PRMT against an aligned pair that holds its second
+// byte in byte 0 and a zero in byte 1 (or, for P_6, its first byte in byte 2 and a zero in byte 1)
 __device__ __forceinline__ Pairs split_pairs(uint32_t wl, uint32_t w0, uint32_t w1, uint32_t wr) {
   Pairs p;
-  uint32_t sm1 = __funnelshift_r(wl, w0, 24);  // bytes x-1 .. x+2
-  uint32_t s2 = __funnelshift_r(w0, w1, 16);   // bytes x+2 .. x+5
-  uint32_t s6 = __funnelshift_r(w1, wr, 16);   // bytes x+6 .. x+9
-  p.m1 = sm1 & 0x00FF00FFu;
-  p.p0 = w0 & 0x00FF00FFu;
-  p.p1 = prmt(w0, 0, 0x4341);
-  p.p2 = s2 & 0x00FF00FFu;
-  p.p3 = prmt(s2, 0, 0x4341);
-  p.p4 = w1 & 0x00FF00FFu;
-  p.p5 = prmt(w1, 0, 0x4341);
-  p.p6 = s6 & 0x00FF00FFu;
+  p.p0 = w0 & 0x00FF00FFu;            // (x,   x+2)
+  p.p1 = prmt(w0, 0, 0x4341);         // (x+1, x+3)
+  p.p4 = w1 & 0x00FF00FFu;            // (x+4, x+6)
+  p.p5 = prmt(w1, 0, 0x4341);         // (x+5, x+7)
+  p.m1 = prmt(wl, p.p1, 0x5453);      // (x-1, x+1): byte 3 of wl, byte 0 of P_1
+  p.p2 = prmt(w0, p.p4, 0x5452);      // (x+2, x+4): byte 2 of w0, byte 0 of P_4
+  p.p3 = prmt(w0, p.p5, 0x5453);      // (x+3, x+5): byte 3 of w0, byte 0 of P_5
+  p.p6 = prmt(p.p4, wr, 0x1412);      // (x+6, x+8): byte 2 of P_4, byte 0 of wr
   return p;
 }
 
