@@ -137,7 +137,18 @@ k_resize(uint8_t *__restrict__ dst, unsigned dw, unsigned dh, const uint8_t *__r
 // 4 address adds + 4 loads per pixel.  (Staging with ordinary loads was tried first: the index arithmetic per
 // staged word cost more than the gathers it replaced.)  Same fp32 evaluation
 // as k_resize.  Used when the rectangle fits (ratios up to about 2.8 : 1 per axis, all up-scalings) and TMA applies.
+//
+// The host sizes the rectangle from the ratio r = s / d with a fixed spare: 127 * rx + 22 columns, 63 * ry + 6 rows.
+// That spare holds for source sizes below RT_SRC_LIMIT.  There every fp32 sx is within 7/8 of
+// (x + 0.5) * s / (float)d - 0.5, whose (float)d is common to the whole tile: sx < 2^22, so the relative roundings of
+// (float)x and x + 0.5 (1.5 * 2^-24 together) and of the product (2^-24) move it by at most 3/8 and 1/4, and the
+// division and the subtraction by half an ulp, 1/8, each.  So a tile's last tap starts less than 127 * rx + 2.75
+// columns (63 * ry + 2.75 rows) after its first, and the rectangle, a1 + 2 - (a0 & ~15) < 127 * rx + 19.75 columns
+// and a1 + 2 - a0 < 63 * ry + 4.75 rows, fits the box.  Past 2^22 the error grows with s until the spare runs out:
+// a 13,162,541-row source resized to 12,210,337 rows needs 74 rows where the box has 73.  Larger sources take
+// k_resize, which stages nothing.  tests/test_resize_geometry.py checks every tile on sweeps of sizes.
 constexpr int RT_MAX_BYTES = 64 * 1024;
+constexpr int RT_SRC_LIMIT = 1 << 22;
 
 template <bool VEC>
 __global__ void __launch_bounds__(256)
@@ -161,7 +172,8 @@ k_resize_tiled(const __grid_constant__ CUtensorMap tmap, uint8_t *__restrict__ d
     resize_axis(y0, sh, dh, a0, b0, f);
     resize_axis(min(y0 + 8u * RS_ROWS - 1, dh - 1), sh, dh, a1, b1, f);
     s_reg[0] = cxa, s_reg[1] = a0;
-    if (cols > pitch || a1 + 2 - a0 > max_rows) __trap();   // the host's bound covers the tile (with spare); never silently wrong
+    // the host's box covers every tile of a source below RT_SRC_LIMIT in both dimensions (proof above); never silently wrong
+    if (cols > pitch || a1 + 2 - a0 > max_rows) __trap();
     mbar_init(&bar, 1);
     mbar_fence_init();
   }
@@ -250,7 +262,8 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
   // Exact 2:1 in both axes: sx = ((x + 0.5) * 2dw) / dw - 0.5 = 2x + 0.5 with every fp32 step exact while
   // (2x + 1) * dw < 2^24, so all four weights are 0.25, the products and their sum are exact, and the truncated
   // result is (a + b + c + d) / 4 -- gs_downsample's arithmetic (reference :189-197), bit for bit.  Checked against
-  // the oracle's literal fp32 evaluation in tests/test_gpu_parity.py::test_stencils_vs_oracle (w/2, h/2 targets).
+  // the oracle's literal fp32 evaluation in tests/test_gpu_parity.py::test_stencils_vs_oracle (w/2, h/2 targets); the
+  // bound is tight: dw = 2897 is the first size whose fp32 map is not 2x + 0.5 (tests/test_resize_geometry.py).
   if (sw == 2 * dw && sh == 2 * dh && (unsigned long long)(2 * dw) * dw < (1ull << 24) &&
       (unsigned long long)(2 * dh) * dh < (1ull << 24) && !gsb::force_generic())
     return gs_b200_downsample_batch(dst, src, sw, sh, n, s);
@@ -258,9 +271,10 @@ int gs_b200_resize_batch(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *
   dim3 grid((dw + 127) / 128, 1, n < gsb::GRID_FRAMES ? n : gsb::GRID_FRAMES);
   const bool aligned8 = sw % 8 == 0 && reinterpret_cast<uintptr_t>(src) % 8 == 0;   // every source row 8-byte aligned
   const bool vec_dst = dw % 4 == 0 && reinterpret_cast<uintptr_t>(dst) % 4 == 0;
-  {
+  if (sw < (unsigned)gsb::RT_SRC_LIMIT && sh < (unsigned)gsb::RT_SRC_LIMIT) {
     // staged-tile kernel: bound the source rectangle of a 128 x 64 dst tile (+3 columns of alignment slack, +2 rows / columns
-    // of neighbours) and use it when it fits the shared-memory budget
+    // of neighbours) and use it when it fits the shared-memory budget.  Below the size limit the ratios are below 2^22,
+    // so the conversions to unsigned below stay in range.
     const double rx = (double)sw / dw, ry = (double)sh / dh;
     const unsigned cols = (unsigned)(127.0 * rx) + 22, rows = (unsigned)((8.0 * gsb::RS_ROWS - 1) * ry) + 6;   // spare: fp32 vs double, 16-byte alignment
     const unsigned pitch = (cols + 15) / 16 * 16;

@@ -129,6 +129,10 @@ GSO_API void gso_resize(uint8_t *dst, unsigned dw, unsigned dh, const uint8_t *s
       unsigned x0 = (unsigned)fx, y0 = (unsigned)fy;
       unsigned x1 = x0 + 1 < sw - 1 ? x0 + 1 : sw - 1, y1 = y0 + 1 < sh - 1 ? y0 + 1 : sh - 1;
       float dx = fx - (float)x0, dy = fy - (float)y0;
+      /* Above 2^24, (float)sw - 1.0f can round to sw or past it, and the reference then reads past the row (column).
+       * Here that tap is the last pixel; dx (dy) is 0 there, so the result is the last pixel's value. */
+      x0 = x0 < sw - 1 ? x0 : sw - 1;
+      y0 = y0 < sh - 1 ? y0 : sh - 1;
       float c00 = src[(size_t)y0 * sw + x0], c01 = src[(size_t)y0 * sw + x1];
       float c10 = src[(size_t)y1 * sw + x0], c11 = src[(size_t)y1 * sw + x1];
       volatile float omx = 1 - dx, omy = 1 - dy;

@@ -1,6 +1,7 @@
 """ctypes loaders shared by the tests: the oracle restatement and numpy wrappers of its calls, the real reference build
 (oracle/_ref, when present), synthetic-input generators and the built library's SASS.  TEST INFRASTRUCTURE only."""
 import ctypes as C
+import glob
 import os
 import re
 import shutil
@@ -449,6 +450,19 @@ def sass_functions():
                 funcs[kernel_id(name)] = arch + "\n" + body
         _cache["sass"] = funcs
     return _cache["sass"]
+
+
+def tile_constants():
+    """{name: value} of the csrc/ `constexpr int NAME = expr;` constants (expressions over earlier ones)"""
+    out = {}
+    for path in sorted(glob.glob(os.path.join(ROOT, "grayskull_b200", "csrc", "*.cu*"))):
+        with open(path) as f:
+            for name, expr in re.findall(r"constexpr\s+(?:unsigned\s+)?int\s+(\w+)\s*=\s*([^;]+);", f.read()):
+                try:
+                    out[name] = int(eval(expr.replace("u", ""), {}, dict(out)))
+                except (NameError, SyntaxError, TypeError):
+                    pass
+    return out
 
 
 # ---- the reference's gs_crop and gs_resize_nn, restated (tests/test_roi.py) ----------------------------------------------

@@ -400,19 +400,6 @@ GRID = 65535
 BAND = 24
 
 
-def tile_constants():
-    """{name: value} of the csrc/ `constexpr int NAME = expr;` constants (expressions over earlier ones)"""
-    out = {}
-    for path in sorted(glob.glob(os.path.join(L.ROOT, "grayskull_b200", "csrc", "*.cu*"))):
-        with open(path) as f:
-            for name, expr in re.findall(r"constexpr\s+(?:unsigned\s+)?int\s+(\w+)\s*=\s*([^;]+);", f.read()):
-                try:
-                    out[name] = int(eval(expr.replace("u", ""), {}, dict(out)))
-                except (NameError, SyntaxError, TypeError):
-                    pass
-    return out
-
-
 # (sym, kernels, geometry without its tall key, tall key, rows of that key per old row tile, the first row of the
 # first old row tile, extra rows of that key beyond its old limit (th - 1: the template's), the tall value)
 def tall(sym, kernels, key, tile, first, past, extra=0, **g):
@@ -486,7 +473,7 @@ TALL_CONTROLS = [row(s, k, **dict(g, h=524_300)) for s, k, g in [
 def test_tall_rows_cross_their_old_limit():
     """each row's tall value passes its site's old limit, with a partial last tile, read from the tile constants in
     csrc/: a retuned tile height cannot move the limit past the test unnoticed"""
-    c = tile_constants()
+    c = L.tile_constants()
     assert {"BX_TH", "BS_TH", "F2_TH", "RS_ROWS", "F3_ROWS"} <= set(c), sorted(c)
     for row in TALL:
         sym, kernels, g, key, tile, first, extra, past = row
@@ -593,7 +580,7 @@ def test_tall_frame(lib, O, witness, row_, which):
     module docstring's table"""
     _room(4)
     sym, kernels, g0, key, tile, first, extra, past = row_
-    c = tile_constants()
+    c = L.tile_constants()
     g = tall_geometry(row_, c, which)
     seams = [first + GRID * tile(c)]
     run_tall(lib, O, witness, sym, kernels, g, seams, "%s %s=%d" % (tall_id(row_), key, g[key]))
