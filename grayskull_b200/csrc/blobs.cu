@@ -22,6 +22,8 @@
 //                   atomic group per (32-pixel word, label)
 //   k_blob_compact  blobs[0..m) in label order, centroid = sums / area in unsigned arithmetic (:397-398)
 // Entries of `blobs` past the returned count are left untouched (the reference leaves first-pass leftovers there).
+#include <climits>
+
 #include "common.cuh"
 #include "scan.cuh"
 
@@ -328,7 +330,8 @@ k_blob_compact(BlobStats st, const unsigned *__restrict__ totals, unsigned nblob
   if (tid == 0) counts[f] = running;
 }
 
-// gs_blob_corners (reference :407-421): one CTA scans the blob's box; lexicographic (value, raster index) minima
+// gs_blob_corners (reference :407-421): one CTA scans the blob's box; lexicographic (value, raster index) minima.
+// Exact for pixels with x + y < 2^31, where the reference's int sums and differences do not overflow.
 __global__ void __launch_bounds__(256)
 k_blob_corners(const uint8_t *__restrict__ img, unsigned w, unsigned h, const uint16_t *__restrict__ labels,
                const BlobRec *__restrict__ blob, unsigned *__restrict__ out /* 4 points */) {
@@ -338,17 +341,23 @@ k_blob_corners(const uint8_t *__restrict__ img, unsigned w, unsigned h, const ui
   if (threadIdx.x < 4) best[threadIdx.x] = ~0ull;
   __syncthreads();
   unsigned long long mine[4] = {~0ull, ~0ull, ~0ull, ~0ull};
-  const unsigned long long cells = (unsigned long long)bw * bh;
+  // the box's part inside the frame.  The reference's loop bounds box.x + box.w and box.y + box.h are 32-bit sums:
+  // a box whose end wraps past 2^32 visits nothing.
+  const unsigned xe = bx + bw, ye = by + bh;
+  const unsigned cw = xe < bx || bx >= w ? 0u : min(xe, w) - bx, ch = ye < by || by >= h ? 0u : min(ye, h) - by;
+  const unsigned long long cells = (unsigned long long)cw * ch;
   for (unsigned long long i = threadIdx.x; i < cells; i += blockDim.x) {
-    const unsigned x = bx + (unsigned)(i % bw), y = by + (unsigned)(i / bw);
-    if (x >= w || y >= h) continue;
+    const unsigned x = bx + (unsigned)(i % cw), y = by + (unsigned)(i / cw);
     const size_t p = (size_t)y * w + x;
     if (img[p] < 128 || labels[p] != label) continue;
     const int sum = (int)x + (int)y, diff = (int)x - (int)y;
     const int v[4] = {sum, -diff, -sum, diff};          // tl: min sum, tr: max diff, br: max sum, bl: min diff
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      const unsigned long long key = ((unsigned long long)(unsigned)(v[q] + 0x40000000) << 32) | (unsigned)p;
+      // tl and bl start from INT_MAX in the reference, and only a smaller value replaces it
+      if ((q == 0 || q == 3) && v[q] == INT_MAX) continue;
+      // flipping the sign bit orders every int as unsigned; w * h < 2^32 keeps p below 2^32 - 1, so no key is ~0
+      const unsigned long long key = ((unsigned long long)((unsigned)v[q] ^ 0x80000000u) << 32) | (unsigned)p;
       mine[q] = key < mine[q] ? key : mine[q];
     }
   }
@@ -386,7 +395,8 @@ k_perspective(uint8_t *__restrict__ dst, unsigned dw, unsigned dh, const uint8_t
       Quad q = q0;
       if (corners) {
 #pragma unroll
-        for (int i = 0; i < 4; i++) q.x[i] = (float)corners[f * 8 + 2 * i], q.y[i] = (float)corners[f * 8 + 2 * i + 1];
+        for (int i = 0; i < 4; i++)
+          q.x[i] = (float)corners[(size_t)f * 8 + 2 * i], q.y[i] = (float)corners[(size_t)f * 8 + 2 * i + 1];
       }
       const float top_x = __fadd_rn(__fmul_rn(q.x[0], omu), __fmul_rn(q.x[1], u));
       const float top_y = __fadd_rn(__fmul_rn(q.y[0], omu), __fmul_rn(q.y[1], u));
@@ -402,8 +412,13 @@ k_perspective(uint8_t *__restrict__ dst, unsigned dw, unsigned dh, const uint8_t
       const unsigned x1 = min(x0 + 1, sw - 1), y1 = min(y0 + 1, sh - 1);
       const float dx = __fsub_rn(sx, (float)x0), dy = __fsub_rn(sy, (float)y0);
       const uint8_t *s = src + (size_t)f * sw * sh;
-      const float c00 = (float)s[(size_t)y0 * sw + x0], c01 = (float)s[(size_t)y0 * sw + x1];
-      const float c10 = (float)s[(size_t)y1 * sw + x0], c11 = (float)s[(size_t)y1 * sw + x1];
+      // the reference samples through gs_get, which gives 0 outside the image.  For about half the sizes above 2^24,
+      // (float)sw - 1.0f rounds past sw - 1, so x0 can be sw or more (y0 likewise); x1 and y1 stay inside.
+      const bool in_x = x0 < sw, in_y = y0 < sh;
+      const float c00 = in_x && in_y ? (float)s[(size_t)y0 * sw + x0] : 0.0f;
+      const float c01 = in_y ? (float)s[(size_t)y0 * sw + x1] : 0.0f;
+      const float c10 = in_x ? (float)s[(size_t)y1 * sw + x0] : 0.0f;
+      const float c11 = (float)s[(size_t)y1 * sw + x1];
       const float omx = __fsub_rn(1.0f, dx), omy = __fsub_rn(1.0f, dy);
       float acc = __fmul_rn(__fmul_rn(c00, omx), omy);
       acc = __fadd_rn(acc, __fmul_rn(__fmul_rn(c01, dx), omy));

@@ -139,7 +139,8 @@ int gs_b200_find_best_match_batch(struct gs_point *best, const uint8_t *result, 
  * w * h < 2^32 - 1. */
 int gs_b200_blobs_batch(const uint8_t *img, unsigned w, unsigned h, unsigned n, gs_label *labels,
                         struct gs_blob *blobs, unsigned *counts, unsigned nblobs, gs_b200_stream s);
-/* gs_blob_corners, reference grayskull.h:407-421: `blob` and `corners` (4 points: tl, tr, br, bl) in DEVICE memory */
+/* gs_blob_corners, reference grayskull.h:407-421: `blob` and `corners` (4 points: tl, tr, br, bl) in DEVICE memory.
+ * Exact for blob pixels with x + y < 2^31; past that the reference's int arithmetic overflows. */
 int gs_b200_blob_corners(const uint8_t *img, unsigned w, unsigned h, const gs_label *labels,
                          const struct gs_blob *blob, struct gs_point *corners, gs_b200_stream s);
 /* gs_perspective_correct, reference grayskull.h:423-444, n source frames -> n dst frames.  per_frame == 0: corners =

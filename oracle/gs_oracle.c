@@ -14,6 +14,7 @@
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may load this file's
  * shared object; the product path (grayskull_b200/) never does.
  */
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -790,20 +791,23 @@ GSO_API unsigned gso_blobs(const uint8_t *img, unsigned w, unsigned h, gs_label 
 
 /* gs_blob_corners, grayskull.h:407-421: over the blob's box, pixels >= 128 carrying its label; the four extremes of
  * x+y (min -> tl, max -> br) and x-y (min -> bl, max -> tr), the FIRST pixel in raster order on ties (strict
- * comparisons); all four default to the centroid.  Restated as key minima: (value, raster index). */
+ * comparisons); all four default to the centroid.  Restated as key minima: (value, raster index), in 64 bits from the
+ * reference's starting values (INT_MAX for the minima, INT_MIN for the maxima): a pixel whose x + y (x - y) is INT_MAX
+ * leaves tl (bl) at the centroid. */
 GSO_API void gso_blob_corners(const uint8_t *img, unsigned w, unsigned h, const gs_label *labels, const struct gs_blob *b,
                               struct gs_point c[4]) {
   long long best[4] = {-1, -1, -1, -1};
-  int val[4] = {0, 0, 0, 0};
+  long long val[4] = {INT_MAX, -(long long)INT_MIN, -(long long)INT_MIN, INT_MAX};
   (void)h;
   for (unsigned y = b->box.y; y < b->box.y + b->box.h; y++)
     for (unsigned x = b->box.x; x < b->box.x + b->box.w; x++) {
       if (x >= w || y >= h || img[(size_t)y * w + x] < 128 || labels[(size_t)y * w + x] != b->label) continue;
       int sum = (int)x + (int)y, diff = (int)x - (int)y;
       long long idx = (long long)y * w + x;
-      int cand[4] = {sum, -diff, -sum, diff};        /* tl: min sum, tr: max diff, br: max sum, bl: min diff */
+      /* tl: min sum, tr: max diff, br: max sum, bl: min diff */
+      long long cand[4] = {sum, -(long long)diff, -(long long)sum, diff};
       for (int k = 0; k < 4; k++)
-        if (best[k] < 0 || cand[k] < val[k]) best[k] = idx, val[k] = cand[k];
+        if (cand[k] < val[k]) best[k] = idx, val[k] = cand[k];
     }
   for (int k = 0; k < 4; k++) {
     if (best[k] < 0) c[k] = b->centroid;
@@ -838,8 +842,11 @@ GSO_API void gso_perspective_correct(uint8_t *dst, unsigned dw, unsigned dh, con
       unsigned x0 = (unsigned)fx, y0 = (unsigned)fy;
       unsigned x1 = x0 + 1 < sw - 1 ? x0 + 1 : sw - 1, y1 = y0 + 1 < sh - 1 ? y0 + 1 : sh - 1;
       volatile float dx = fx - (float)x0, dy = fy - (float)y0;
-      float c00 = src[(size_t)y0 * sw + x0], c01 = src[(size_t)y0 * sw + x1];
-      float c10 = src[(size_t)y1 * sw + x0], c11 = src[(size_t)y1 * sw + x1];
+      /* gs_get's 0 outside the image: above 2^24, (float)sw - 1.0f can round past sw - 1, putting x0 at sw or
+       * beyond (y0 likewise); x1 and y1 are clamped to the last pixel */
+      int in_x = x0 < sw, in_y = y0 < sh;
+      float c00 = in_x && in_y ? src[(size_t)y0 * sw + x0] : 0, c01 = in_y ? src[(size_t)y0 * sw + x1] : 0;
+      float c10 = in_x ? src[(size_t)y1 * sw + x0] : 0, c11 = src[(size_t)y1 * sw + x1];
       volatile float omx = 1 - dx, omy = 1 - dy;
       volatile float t0 = c00 * omx, t1 = c01 * dx, t2 = c10 * omx, t3 = c11 * dx;
       t0 = t0 * omy;
