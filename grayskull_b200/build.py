@@ -1,5 +1,5 @@
-"""Build libgrayskull_b200.so and its companion libgrayskull_draw.so in-tree with nvcc for sm_90a (H100; cross-compiles
-without a GPU), and the gsb_magick CLI on both.
+"""Build libgrayskull_b200.so and its companions libgrayskull_draw.so and libgrayskull_contour.so in-tree with nvcc for
+sm_90a (H100; cross-compiles without a GPU), and the gsb_magick CLI on all three.
 
     python -m grayskull_b200.build            # incremental
     python -m grayskull_b200.build --force
@@ -25,6 +25,10 @@ SOURCES = ["runtime.cu", "stencil3.cu", "box.cu", "resample.cu", "integral.cu", 
 DRAW_DIR = os.path.join(HERE, "draw")
 DRAW_LIB = os.path.join(HERE, "libgrayskull_draw.so")
 DRAW_SOURCES = ["draw.cu"]
+# the companion library of contour tracing (include/grayskull_contour.h), built the same way
+CONTOUR_DIR = os.path.join(HERE, "contour")
+CONTOUR_LIB = os.path.join(HERE, "libgrayskull_contour.so")
+CONTOUR_SOURCES = ["contour.cu"]
 CASCADE_NPZ = os.path.join(HERE, "data", "frontalface.npz")
 CASCADE_H = os.path.join(OBJ, "frontalface_cascade.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -42,9 +46,10 @@ def nvcc():
 def _deps_mtime():
     files = [os.path.join(CSRC, f) for f in os.listdir(CSRC)]
     files += [os.path.join(DRAW_DIR, f) for f in os.listdir(DRAW_DIR)]
+    files += [os.path.join(CONTOUR_DIR, f) for f in os.listdir(CONTOUR_DIR)]
     files += [os.path.join(os.path.dirname(HERE), "include", f)
               for f in ("grayskull.h", "grayskull_b200.h", "grayskull_b200_roi.h", "grayskull_b200_pyramid.h",
-                        "grayskull_draw.h")]
+                        "grayskull_draw.h", "grayskull_contour.h")]
     files += [os.path.join(HERE, "cli", "gsb_magick.c"), CASCADE_NPZ]
     return max(os.path.getmtime(f) for f in files)
 
@@ -52,7 +57,7 @@ def _deps_mtime():
 def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
     newest = _deps_mtime()
-    if not force and all(os.path.exists(p) and os.path.getmtime(p) >= newest for p in (LIB, DRAW_LIB)):
+    if not force and all(os.path.exists(p) and os.path.getmtime(p) >= newest for p in (LIB, DRAW_LIB, CONTOUR_LIB)):
         if not os.path.exists(os.path.join(HERE, "gsb_magick")):
             build_cli()
         return LIB
@@ -71,9 +76,12 @@ def build(force=False, verbose=False):
         return obj
 
     draw_srcs = [os.path.join(DRAW_DIR, f) for f in DRAW_SOURCES]   # absolute: os.path.join keeps them as they are
-    with ThreadPoolExecutor(max_workers=min(8, len(SOURCES) + len(draw_srcs))) as ex:
-        all_objs = list(ex.map(compile_one, SOURCES + draw_srcs))
-    objs, draw_objs = all_objs[:len(SOURCES)], all_objs[len(SOURCES):]
+    contour_srcs = [os.path.join(CONTOUR_DIR, f) for f in CONTOUR_SOURCES]
+    with ThreadPoolExecutor(max_workers=min(8, len(SOURCES) + len(draw_srcs) + len(contour_srcs))) as ex:
+        all_objs = list(ex.map(compile_one, SOURCES + draw_srcs + contour_srcs))
+    objs = all_objs[:len(SOURCES)]
+    draw_objs = all_objs[len(SOURCES):len(SOURCES) + len(draw_srcs)]
+    contour_objs = all_objs[len(SOURCES) + len(draw_srcs):]
     # export only the C ABI (gs_*); C++ symbols stay local
     vs = os.path.join(OBJ, "exports.map")
     with open(vs, "w") as f:
@@ -82,11 +90,12 @@ def build(force=False, verbose=False):
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout + r.stderr)
-    # the companion: its own static cudart, the same export rule
-    r = subprocess.run([cc, "-shared", "-o", DRAW_LIB] + draw_objs + ["-Xlinker", "--version-script=" + vs],
-                       capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("link of %s failed:\n%s" % (os.path.basename(DRAW_LIB), r.stdout + r.stderr))
+    # the companions: each its own static cudart, the same export rule
+    for lib, lib_objs in ((DRAW_LIB, draw_objs), (CONTOUR_LIB, contour_objs)):
+        r = subprocess.run([cc, "-shared", "-o", lib] + lib_objs + ["-Xlinker", "--version-script=" + vs],
+                           capture_output=True, text=True)
+        if r.returncode != 0:
+            raise RuntimeError("link of %s failed:\n%s" % (os.path.basename(lib), r.stdout + r.stderr))
     build_cli()
     return LIB
 
@@ -117,13 +126,14 @@ def write_cascade_header():
 
 
 def build_cli():
-    """gsb_magick: the C99 batch-pipeline CLI on the device-resident ABI (cli/gsb_magick.c), on both libraries"""
+    """gsb_magick: the C99 batch-pipeline CLI on the device-resident ABI (cli/gsb_magick.c), on all three libraries"""
     exe = os.path.join(HERE, "gsb_magick")
     write_cascade_header()
     cmd = ["gcc", "-std=c99", "-O2", "-Wall", "-Wextra", "-Werror", "-pedantic", "-D_POSIX_C_SOURCE=200809L",
            "-I", os.path.join(os.path.dirname(HERE), "include"), "-I", OBJ, "-o", exe,
            os.path.join(HERE, "cli", "gsb_magick.c"),
-           "-L" + HERE, "-l:" + os.path.basename(DRAW_LIB), "-l:" + os.path.basename(LIB), "-Wl,-rpath,$ORIGIN"]
+           "-L" + HERE, "-l:" + os.path.basename(DRAW_LIB), "-l:" + os.path.basename(CONTOUR_LIB),
+           "-l:" + os.path.basename(LIB), "-Wl,-rpath,$ORIGIN"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("gsb_magick build failed:\n" + r.stdout + r.stderr)

@@ -109,6 +109,11 @@ struct gs_blob {
   struct gs_rect box;
   struct gs_point centroid;
 };
+struct gs_contour { /* traced on the device by include/grayskull_contour.h */
+  struct gs_rect box;
+  struct gs_point start;
+  unsigned length;
+};
 struct gs_keypoint {
   struct gs_point pt;
   unsigned response;
