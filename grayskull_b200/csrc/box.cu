@@ -1278,7 +1278,13 @@ int gs_b200_blur_sobel_batch(uint8_t *dst, const uint8_t *src, unsigned w, unsig
     int ctas = 0;
     if (int rc = gsb::blur_sobel_ctas_per_sm(radius, reinterpret_cast<const void *>(k), &ctas)) return rc;
     // resident CTAs only; each takes its next tile from a counter, so the tiles in flight stay one raster window
-    const unsigned long long resident = (unsigned long long)ctas * gsb::sm_count(), grid = tiles < resident ? tiles : resident;
+    const unsigned long long resident = (unsigned long long)ctas * gsb::sm_count();
+    unsigned long long grid = tiles < resident ? tiles : resident;
+    // test hook: GS_B200_BLUR_SOBEL_CTAS=k launches at most k CTAs, so that a CTA makes edge tiles after other tiles
+    if (const char *ce = getenv("GS_B200_BLUR_SOBEL_CTAS")) {
+      const long long k = atoll(ce);
+      if (k >= 1 && (unsigned long long)k < grid) grid = (unsigned long long)k;
+    }
     unsigned *taken = static_cast<unsigned *>(gsb::workspace(s, gsb::WS_BLUR_SOBEL_TILES, sizeof(unsigned)));
     if (!taken) return gsb::workspace_error();
     GSB_CHECK(cudaMemsetAsync(taken, 0, sizeof(unsigned), s));

@@ -5,7 +5,7 @@ use by name, fixtures included (`from _gpu import G, lib, witness  # noqa: F401`
     probe: whether torch.profiler sees the library's launches at all);
   * dev(), stream(), Region (a view into a guarded device allocation), frames() (a seeded batch);
   * traced() runs one call under torch.profiler and returns the kernels it launched; witnessed() checks a case's
-    kernels among them."""
+    kernels among them; traced_grids() returns the grid of each launch of one kernel."""
 import ctypes as C
 import os
 
@@ -19,7 +19,8 @@ from _libs import kernel_id
 # Without it, once a process has run some sessions, later ones intermittently deliver no kernel records or only their
 # last kernels (on an H100: 3 of 3 witness probes and 443 sessions of one run of the GPU suite, with every output
 # bit-exact); with it, every session of the same run recorded all its kernels.  Set at import, before the first
-# session of the process: every module that traces imports this one, and every session runs through traced().
+# session of the process: every module that traces imports this one, and every session runs through traced() or
+# traced_grids().
 os.environ.setdefault("TEARDOWN_CUPTI", "1")
 
 
@@ -107,6 +108,27 @@ def traced(fn):
     mangled = sorted(nm for nm in names if nm.startswith("_Z"))
     names = (names - set(mangled)) | set(L.demangle(mangled))
     return rc, {kernel_id(nm) for nm in names if "gsb::" in nm}
+
+
+def traced_grids(fn, kernel):
+    """run fn() under torch.profiler with CUDA activity -> (its result, the grid (x, y, z) of each launch of a kernel
+    whose name contains `kernel`, in launch order), read from the session's trace"""
+    import json
+    import tempfile
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        out = fn()
+        torch.cuda.synchronize()
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "trace.json")
+        prof.export_chrome_trace(path)
+        with open(path) as f:
+            events = json.load(f)["traceEvents"]
+    launches = sorted((e for e in events if e.get("cat") == "kernel" and kernel in e.get("name", "")),
+                      key=lambda e: e["ts"])
+    return out, [tuple(e["args"]["grid"]) for e in launches]
 
 
 @pytest.fixture(scope="module")
