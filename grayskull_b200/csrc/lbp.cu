@@ -44,9 +44,13 @@ namespace gsb {
 struct ScaleInfo {
   int win_w, win_h, nx, ny;
   unsigned chunks;             // 32-window slots per scan row
-  unsigned feat_off;           // first entry of this scale in the feature table
+  unsigned feat_off;           // first entry of this scale's geometry in feat / geo / tgeo (shared by equal scales)
   unsigned long long slot0;    // first slot of this scale (a multiple of LBP_SLOTS_PER_CTA)
 };
+// Longest ladder gs_b200_lbp_detect_batch scans; a longer one is an error (cudaErrorInvalidValue), never a shorter
+// list.  65536 scales hold any scale_factor >= 1.0001 over a 700x range of scales; scale_factor = 1 + 2^-23 needs
+// millions.  A scale costs 32 B of tables, 512 B of hit masks per frame and one CTA of the scan.
+constexpr int LBP_MAX_SCALES = 65536;
 struct FeatGeo {               // corner lattice of one feature at one scale, as element offsets
   int row[4];                  // (fy - 1 + j*fh) * iw
   int col[4];                  // fx - 1 + i*fw
@@ -90,6 +94,17 @@ struct DevCascade {            // pointers into one device blob
   int step;
   bool safe_geometry;          // every feature stays inside its window at every scale
 };
+
+// the scale that owns `slot`: the last one with slot0 <= slot (slot0 grows strictly, every scale has slots)
+__device__ __forceinline__ int scale_of(const DevCascade &dc, unsigned long long slot) {
+  int lo = 0, hi = dc.nscales - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (dc.scales[mid].slot0 <= slot) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
 
 template <bool GUARD>
 __device__ __forceinline__ uint32_t corner(const uint32_t *__restrict__ ii, unsigned iw, unsigned ih, int x, int y) {
@@ -152,9 +167,7 @@ k_lbp_scan(const uint32_t *__restrict__ ii_all, unsigned iw, unsigned ih, DevCas
   const uint32_t *ii = ii_all + (size_t)f * iw * ih;
   unsigned mask = 0;
   if (slot < dc.total_slots) {
-    int si = 0;
-    while (si + 1 < dc.nscales && slot >= dc.scales[si + 1].slot0) si++;
-    const ScaleInfo sc = dc.scales[si];
+    const ScaleInfo sc = dc.scales[scale_of(dc, slot)];
     const unsigned long long rel = slot - sc.slot0;
     const unsigned yi = (unsigned)(rel / sc.chunks), xi = (unsigned)(rel % sc.chunks) * 32 + lane;
     const bool valid = xi < (unsigned)sc.nx && yi < (unsigned)sc.ny;   // padding slots are empty
@@ -230,15 +243,13 @@ k_lbp_scan2(const uint32_t *__restrict__ ii_all, unsigned iw, unsigned ih, DevCa
   const unsigned long long slot_first = (unsigned long long)blockIdx.x * LBP_SLOTS_PER_CTA;
   const uint32_t *ii = ii_all + (size_t)f * iw * ih;
   if (tid == 0) {
-    int si = 0;
-    while (si + 1 < dc.nscales && slot_first >= dc.scales[si + 1].slot0) si++;
-    s_scale = si;
+    s_scale = scale_of(dc, slot_first);
     cnt[0] = cnt[1] = 0;
   }
   __syncthreads();
   const ScaleInfo sc = dc.scales[s_scale];
   {  // tables -> shared memory (word copies)
-    const uint32_t *g0 = reinterpret_cast<const uint32_t *>(dc.geo + (size_t)s_scale * dc.nfeatures);
+    const uint32_t *g0 = reinterpret_cast<const uint32_t *>(dc.geo + sc.feat_off);
     uint32_t *d0 = reinterpret_cast<uint32_t *>(s_geo);
     for (int i = tid; i < dc.nfeatures * 8; i += LBP_THREADS) d0[i] = g0[i];
     const uint32_t *g1 = reinterpret_cast<const uint32_t *>(dc.weaks);
@@ -400,7 +411,7 @@ k_lbp_scan3(const __grid_constant__ CUtensorMap tmap, DevCascade dc, int si, int
     tma_load_3d(tile + plane_bytes, &tmap, wx0 - 4, wy0 * dc.step - 1, 2 * (int)f + 1, &bar);
   }
   {  // tables -> shared memory while the boxes are in flight
-    const uint32_t *g0 = reinterpret_cast<const uint32_t *>(dc.tgeo + (size_t)si * dc.nfeatures);
+    const uint32_t *g0 = reinterpret_cast<const uint32_t *>(dc.tgeo + sc.feat_off);
     uint32_t *d0 = reinterpret_cast<uint32_t *>(s_geo);
     for (int i = tid; i < dc.nfeatures * 8; i += LBP3_THREADS) d0[i] = g0[i];
     const uint32_t *g1 = reinterpret_cast<const uint32_t *>(dc.weaks);
@@ -610,9 +621,7 @@ k_lbp_emit(DevCascade dc, const unsigned *__restrict__ masks, const unsigned *__
       const unsigned p = pos + __popc(m & ((1u << lane) - 1u));
       if (p < max_rects) {
         const unsigned long long slot = slot0 + i;
-        int si = 0;
-        while (si + 1 < dc.nscales && slot >= dc.scales[si + 1].slot0) si++;
-        const ScaleInfo sc = dc.scales[si];
+        const ScaleInfo sc = dc.scales[scale_of(dc, slot)];
         const unsigned long long rel = slot - sc.slot0;
         const unsigned yi = (unsigned)(rel / sc.chunks), xi = (unsigned)(rel % sc.chunks) * 32 + lane;
         *reinterpret_cast<uint4 *>(rects + (size_t)f * max_rects + p) =
@@ -696,31 +705,46 @@ static unsigned long long cascade_hash(const struct gs_lbp_cascade *c) {
   return h;
 }
 
-// the reference's scale ladder (:819-821), one entry per scale it would scan
-static void build_scales(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih, float scale_factor, float min_scale,
-                         float max_scale, int step, std::vector<float> &scale_vals, std::vector<ScaleInfo> &out) {
-  unsigned long long slot = 0;
+// The reference's scale ladder (:819-821): fn(scale, win_w, win_h) for each scale it scans, until fn returns false.
+// A ladder that does not grow (scale_factor <= 1) ends after its first scale here; the reference repeats that scale
+// until max_rects fills, and never returns when it has no hit.  A NaN scale_factor ends after the first scale in both.
+template <class F>
+static void walk_ladder(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih, float scale_factor, float min_scale,
+                        float max_scale, F fn) {
   for (volatile float scale = min_scale; scale <= max_scale; scale = scale * scale_factor) {
     const float s = scale;
     const int win_w = (int)((float)c->window_w * s), win_h = (int)((float)c->window_h * s);
     if (win_w > (int)iw || win_h > (int)ih) break;
+    if (!fn(s, win_w, win_h) || !(scale_factor > 1.0f)) break;
+  }
+}
+
+// one entry per scale of the ladder; false (and the first LBP_MAX_SCALES entries) when it has more scales than that
+static bool build_scales(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih, float scale_factor, float min_scale,
+                         float max_scale, int step, std::vector<float> &scale_vals, std::vector<ScaleInfo> &out) {
+  unsigned long long slot = 0;
+  bool fits = true;
+  walk_ladder(c, iw, ih, scale_factor, min_scale, max_scale, [&](float s, int win_w, int win_h) {
+    if (out.size() == (size_t)LBP_MAX_SCALES) return fits = false;
     ScaleInfo si;
     si.win_w = win_w, si.win_h = win_h;
     si.nx = ((int)iw - win_w) / step + 1, si.ny = ((int)ih - win_h) / step + 1;
     si.chunks = (unsigned)(si.nx + 31) / 32;
-    si.feat_off = (unsigned)out.size() * c->nfeatures;
+    si.feat_off = 0;   // set with the feature tables (get_plan)
     si.slot0 = slot;
     slot += (unsigned long long)si.chunks * si.ny;
     slot = (slot + LBP_SLOTS_PER_CTA - 1) / LBP_SLOTS_PER_CTA * LBP_SLOTS_PER_CTA;   // CTAs never straddle scales
     out.push_back(si);
     scale_vals.push_back(s);
-    if (out.size() > 4096 || !(scale_factor > 1.0f)) break;  // a non-growing ladder never ends in the reference
-  }
+    return true;
+  });
+  return fits;
 }
 
-// the cached plan of this cascade and geometry; on a miss it is built and uploaded (blocking) unless !may_build
+// the cached plan of this cascade and geometry; on a miss it is built and uploaded (blocking) unless !may_build.
+// nullptr with the recorded error in *err when there is none
 static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih, float sf, float mn, float mx,
-                        int step, bool may_build) {
+                        int step, bool may_build, int *err) {
   int dev = 0;
   cudaGetDevice(&dev);
   // test hook: 1 = every scale on the 1024-thread tile form, 0 = none, unset = by tile height (tests reach both
@@ -730,37 +754,49 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
   std::lock_guard<std::mutex> lock(g_plan_mutex);
   for (auto &r : g_plans)
     if (r->key == key) return r;
-  if (!may_build) return nullptr;
+  if (!may_build) {
+    *err = record_error(cudaErrorStreamCaptureUnsupported, __FILE__, __LINE__);
+    return nullptr;
+  }
 
   PlanRef ref = std::make_shared<PlanEntry>();
   PlanEntry &e = *ref;
   e.key = key;
   std::vector<float> svals;
-  build_scales(c, iw, ih, sf, mn, mx, step, svals, e.scales);
+  if (!build_scales(c, iw, ih, sf, mn, mx, step, svals, e.scales)) {
+    *err = record_error(cudaErrorInvalidValue, __FILE__, __LINE__);   // a ladder of more than LBP_MAX_SCALES scales
+    return nullptr;
+  }
   const int ns = (int)e.scales.size(), nf = c->nfeatures, nw = c->nweaks, nst = c->nstages;
   const unsigned nsub = subsets_len(c);
-  std::vector<short4> feat((size_t)ns * nf);
+  // Neighbouring scales of a long ladder mostly truncate to the same window and features: such a scale scans with
+  // the previous scale's tables (its hits are the same windows again).
+  std::vector<short4> feat;
   bool safe = true;
-  for (int s = 0; s < ns; s++)
+  for (int s = 0; s < ns; s++) {
+    const size_t at = feat.size();
     for (int i = 0; i < nf; i++) {
       const float sc = svals[s];
       int fx = (int)((float)c->features[i * 4 + 0] * sc), fy = (int)((float)c->features[i * 4 + 1] * sc);
       int fw = (int)((float)c->features[i * 4 + 2] * sc), fh = (int)((float)c->features[i * 4 + 3] * sc);
       if (fw < 1) fw = 1;
       if (fh < 1) fh = 1;
-      feat[(size_t)s * nf + i] = make_short4((short)fx, (short)fy, (short)fw, (short)fh);
+      feat.push_back(make_short4((short)fx, (short)fy, (short)fw, (short)fh));
       if (fx < 0 || fy < 0 || fx + 3 * fw > e.scales[s].win_w || fy + 3 * fh > e.scales[s].win_h) safe = false;
     }
-  std::vector<FeatGeo> geo((size_t)ns * nf);
-  for (int s = 0; s < ns; s++)
-    for (int i = 0; i < nf; i++) {
-      const short4 ft = feat[(size_t)s * nf + i];
-      FeatGeo &g = geo[(size_t)s * nf + i];
-      for (int k = 0; k < 4; k++) {
-        g.row[k] = (ft.y - 1 + k * ft.w) * (int)iw;
-        g.col[k] = ft.x - 1 + k * ft.z;
-      }
+    const bool same = s > 0 && e.scales[s].win_w == e.scales[s - 1].win_w && e.scales[s].win_h == e.scales[s - 1].win_h &&
+                      memcmp(feat.data() + at, feat.data() + e.scales[s - 1].feat_off, sizeof(short4) * nf) == 0;
+    if (same) feat.resize(at);
+    e.scales[s].feat_off = same ? e.scales[s - 1].feat_off : (unsigned)at;
+  }
+  std::vector<FeatGeo> geo(feat.size());
+  for (size_t i = 0; i < feat.size(); i++) {
+    const short4 ft = feat[i];
+    for (int k = 0; k < 4; k++) {
+      geo[i].row[k] = (ft.y - 1 + k * ft.w) * (int)iw;
+      geo[i].col[k] = ft.x - 1 + k * ft.z;
     }
+  }
   // window tiles for k_lbp_scan3: per scale the widest tile whose box fits a TMA box (256 elements per
   // dimension) and the tallest one whose box fits the shared-memory budget
   const size_t table_bytes_t = sizeof(TileGeo) * nf + sizeof(Weak) * nw + sizeof(Stage) * nst + 4 * (size_t)nsub;
@@ -816,8 +852,9 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
     tp.tiles_x = (si.nx + tp.twx - 1) / tp.twx, tp.tiles_y = (si.ny + tp.twy - 1) / tp.twy;
     if ((unsigned long long)tp.tiles_x * tp.tiles_y > 0x7FFFFFFFull) tiles_ok = false;
     e.tiles.push_back(tp);
+    if (s2 > 0 && si.feat_off == e.scales[s2 - 1].feat_off) continue;   // the same window: the same tile plan and tgeo
     for (int i = 0; i < nf; i++) {
-      const short4 ft = feat[(size_t)s2 * nf + i];
+      const short4 ft = feat[si.feat_off + i];
       TileGeo g;
       const int plane = (int)((((size_t)tp.bw * tp.ph * 4 + 127) & ~(size_t)127));
       for (int k = 0; k < 4; k++) {
@@ -854,8 +891,11 @@ static PlanRef get_plan(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih
   memcpy(&host[o_sb], c->subsets, 4 * (size_t)nsub);
   memcpy(&host[o_st], stages.data(), sizeof(Stage) * nst);
   if (!geo.empty()) memcpy(&host[o_ge], geo.data(), sizeof(FeatGeo) * geo.size());
-  if (cudaMalloc(&e.blob, total) != cudaSuccess) return nullptr;
-  if (upload(e.blob, host.data(), total, __FILE__, __LINE__)) return nullptr;
+  if (cudaMalloc(&e.blob, total) != cudaSuccess) {
+    *err = record_error(cudaErrorMemoryAllocation, __FILE__, __LINE__);
+    return nullptr;
+  }
+  if ((*err = upload(e.blob, host.data(), total, __FILE__, __LINE__))) return nullptr;
   unsigned char *b = static_cast<unsigned char *>(e.blob);
   e.dc.scales = reinterpret_cast<const ScaleInfo *>(b + o_sc);
   e.dc.feat = reinterpret_cast<const short4 *>(b + o_ft);
@@ -894,11 +934,11 @@ extern "C" {
 unsigned long long gs_b200_lbp_window_count(const struct gs_lbp_cascade *c, unsigned iw, unsigned ih,
                                             float scale_factor, float min_scale, float max_scale, int step) {
   GSB_ASSERT(c && step > 0);
-  std::vector<float> sv;
-  std::vector<gsb::ScaleInfo> sc;
-  gsb::build_scales(c, iw, ih, scale_factor, min_scale, max_scale, step, sv, sc);
   unsigned long long n = 0;
-  for (auto &s : sc) n += (unsigned long long)s.nx * s.ny;
+  gsb::walk_ladder(c, iw, ih, scale_factor, min_scale, max_scale, [&](float, int win_w, int win_h) {
+    n += (unsigned long long)(((int)iw - win_w) / step + 1) * (((int)ih - win_h) / step + 1);
+    return true;
+  });
   return n;
 }
 
@@ -916,8 +956,9 @@ int gs_b200_lbp_detect_batch(const struct gs_lbp_cascade *c, const uint32_t *ii,
   cudaStream_t st = static_cast<cudaStream_t>(s);
   // a plan miss allocates and uploads synchronously, which a graph capture cannot hold
   const bool cap = gsb::capturing(st);
-  gsb::PlanRef p = gsb::get_plan(c, iw, ih, scale_factor, min_scale, max_scale, step, !cap);
-  if (!p) return gsb::record_error(cap ? cudaErrorStreamCaptureUnsupported : cudaErrorMemoryAllocation, __FILE__, __LINE__);
+  int err = 0;
+  gsb::PlanRef p = gsb::get_plan(c, iw, ih, scale_factor, min_scale, max_scale, step, !cap, &err);
+  if (!p) return err;
   const gsb::DevCascade &dc = p->dc;
   if (dc.total_slots == 0 || max_rects == 0) {
     GSB_CHECK(cudaMemsetAsync(counts, 0, sizeof(unsigned) * n, st));
