@@ -3,8 +3,8 @@
  * the hot path).  Plain C99 against include/grayskull.h (stand-alone mode) + include/grayskull_b200.h, linked against
  * libgrayskull_b200.so and, for the draw-* and faces stages, libgrayskull_draw.so (include/grayskull_draw.h), for
  * the contour stage libgrayskull_contour.so (include/grayskull_contour.h), for the contour and scan stages
- * libgrayskull_corners.so (include/grayskull_corners.h), and for colour inputs libgrayskull_color.so
- * (include/grayskull_color.h).
+ * libgrayskull_corners.so (include/grayskull_corners.h), for the faces-grouped stage libgrayskull_group.so
+ * (include/grayskull_group.h), and for colour inputs libgrayskull_color.so (include/grayskull_color.h).
  *
  *   gsb_magick <pipeline> <out-prefix> in0.pgm|in0.ppm [in1 ...]
  *
@@ -26,6 +26,10 @@
  *   faces:N         (the faces verb's picture, nanomagick.c:347-376: LBP detection with the frontalface cascade, at most
  *                    100 rects, scales 1.0..4.0 by 1.2, N minimum neighbours, each rect's outline drawn at 255.  Runs at
  *                    any frame size; the verb refuses frames over 640x480)
+ *   faces-grouped:S:K (faces as groups of windows rather than every window: LBP detection with the frontalface cascade,
+ *                    at most 4096 rects, scales 1.0..4.0 by 1.2, scan step S; then gs_b200_group_rects_batch with
+ *                    min_neighbors K and eps 0.2, and each group's outline drawn at 255; prints "frame F: R windows,
+ *                    G faces")
  *   contour:N       (the reference's wasm demo's gs_detect_largest_blob_contour(src, N), examples/wasm/grayskull.c:
  *                    278-326, per frame: blobs of the frame with N records, the largest (the first on ties) when its
  *                    area is at least 100, its first label pixel in raster order as the start, then gs_trace_contour on
@@ -55,6 +59,7 @@
 #include "grayskull_contour.h"
 #include "grayskull_corners.h"
 #include "grayskull_draw.h"
+#include "grayskull_group.h"
 #include "frontalface_cascade.h" /* generated by build.py from grayskull_b200/data/frontalface.npz */
 
 #define DIE(...) (fprintf(stderr, "gsb_magick: " __VA_ARGS__), fprintf(stderr, "\n"), exit(1))
@@ -73,6 +78,10 @@
 #define CKK(call)                                                              \
   do {                                                                         \
     if ((call) != 0) DIE("%s failed: %s", #call, gs_b200_color_last_error());  \
+  } while (0)
+#define CKG(call)                                                              \
+  do {                                                                         \
+    if ((call) != 0) DIE("%s failed: %s", #call, gs_b200_group_last_error());  \
   } while (0)
 #define CKD(call)                                                             \
   do {                                                                        \
@@ -349,6 +358,39 @@ static void stage(const char *spec, struct batch *cur, struct batch *tmp, size_t
     CKD(gs_b200_draw_rects_batch(tmp->dev, cur->dev, w, h, n, rects, counts, MR, NULL));
     CK(gs_b200_stream_sync(NULL));
     gs_b200_free(ii), gs_b200_free(rects), gs_b200_free(counts);
+  } else if (!strcmp(name, "faces-grouped") && nargs == 2) {
+    /* the faces stage's detection with a real scan step and room for every window, then the windows grouped on the
+     * device (min_neighbors K, eps 0.2), as many frames per chunk as 256 MiB of grouping state holds */
+    enum { MR = 4096 };
+    int step = atoi(a0), k = atoi(a1);
+    unsigned f, *counts, *gcounts, *hc, *hg;
+    uint32_t *ii;
+    struct gs_rect *rects, *groups;
+    size_t wb = gs_b200_group_rects_work_bytes(MR, n), one = gs_b200_group_rects_work_bytes(MR, 1);
+    void *work;
+    if (step <= 0) DIE("scan step must be positive in '%s'", spec);
+    if (k < 0) DIE("minimum neighbors must not be negative in '%s'", spec);
+    if (wb > ((size_t)256 << 20)) wb = one > ((size_t)256 << 20) ? one : ((size_t)256 << 20);
+    ii = (uint32_t *)gs_b200_malloc(sizeof(uint32_t) * frame_bytes(cur) * n);
+    rects = (struct gs_rect *)gs_b200_malloc(sizeof(*rects) * (size_t)MR * n);
+    groups = (struct gs_rect *)gs_b200_malloc(sizeof(*groups) * (size_t)MR * n);
+    counts = (unsigned *)gs_b200_malloc(sizeof(unsigned) * n);
+    gcounts = (unsigned *)gs_b200_malloc(sizeof(unsigned) * n);
+    work = gs_b200_malloc(wb);
+    hc = (unsigned *)malloc(sizeof(unsigned) * n);
+    hg = (unsigned *)malloc(sizeof(unsigned) * n);
+    if (!ii || !rects || !groups || !counts || !gcounts || !work || !hc || !hg) DIE("allocation failed");
+    CK(gs_b200_integral_batch(ii, cur->dev, w, h, n, NULL));
+    CK(gs_b200_lbp_detect_batch(&frontalface, ii, w, h, n, rects, counts, MR, 1.2f, 1.0f, 4.0f, step, NULL));
+    CKG(gs_b200_group_rects_batch(rects, counts, MR, n, (unsigned)k, 0.2, groups, NULL, gcounts, MR, work, wb, NULL));
+    ensure(tmp, w, h, n, cap_tmp);
+    CKD(gs_b200_draw_rects_batch(tmp->dev, cur->dev, w, h, n, groups, gcounts, MR, NULL));
+    CK(gs_b200_memcpy_d2h(hc, counts, sizeof(unsigned) * n, NULL));
+    CK(gs_b200_memcpy_d2h(hg, gcounts, sizeof(unsigned) * n, NULL));
+    CK(gs_b200_stream_sync(NULL));
+    for (f = 0; f < n; f++) printf("frame %u: %u windows, %u faces\n", f, hc[f], hg[f]);
+    gs_b200_free(ii), gs_b200_free(rects), gs_b200_free(groups), gs_b200_free(counts), gs_b200_free(gcounts);
+    gs_b200_free(work), free(hc), free(hg);
   } else if (!strcmp(name, "keypoints") && nargs == 2) {
     unsigned nk = (unsigned)atoi(a0), f, *counts, *hc;
     struct gs_keypoint *kps;
