@@ -1,6 +1,6 @@
 """Build libgrayskull_b200.so and its companions libgrayskull_draw.so, libgrayskull_contour.so, libgrayskull_color.so,
-libgrayskull_corners.so and libgrayskull_group.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU), and
-the gsb_magick CLI on all six.
+libgrayskull_corners.so, libgrayskull_group.so and libgrayskull_homography.so in-tree with nvcc for sm_90a (H100;
+cross-compiles without a GPU), and the gsb_magick CLI on all seven.
 
     python -m grayskull_b200.build            # incremental
     python -m grayskull_b200.build --force
@@ -42,6 +42,10 @@ CORNERS_SOURCES = ["corners.cu"]
 GROUP_DIR = os.path.join(HERE, "group")
 GROUP_LIB = os.path.join(HERE, "libgrayskull_group.so")
 GROUP_SOURCES = ["group.cu"]
+# the companion library of template homographies (include/grayskull_homography.h), built the same way
+HOMOGRAPHY_DIR = os.path.join(HERE, "homography")
+HOMOGRAPHY_LIB = os.path.join(HERE, "libgrayskull_homography.so")
+HOMOGRAPHY_SOURCES = ["homography.cu"]
 CASCADE_NPZ = os.path.join(HERE, "data", "frontalface.npz")
 CASCADE_H = os.path.join(OBJ, "frontalface_cascade.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -63,10 +67,11 @@ def _deps_mtime():
     files += [os.path.join(COLOR_DIR, f) for f in os.listdir(COLOR_DIR)]
     files += [os.path.join(CORNERS_DIR, f) for f in os.listdir(CORNERS_DIR)]
     files += [os.path.join(GROUP_DIR, f) for f in os.listdir(GROUP_DIR)]
+    files += [os.path.join(HOMOGRAPHY_DIR, f) for f in os.listdir(HOMOGRAPHY_DIR)]
     files += [os.path.join(os.path.dirname(HERE), "include", f)
               for f in ("grayskull.h", "grayskull_b200.h", "grayskull_b200_roi.h", "grayskull_b200_pyramid.h",
                         "grayskull_draw.h", "grayskull_contour.h", "grayskull_color.h", "grayskull_corners.h",
-                        "grayskull_group.h")]
+                        "grayskull_group.h", "grayskull_homography.h")]
     files += [os.path.join(HERE, "cli", "gsb_magick.c"), CASCADE_NPZ]
     return max(os.path.getmtime(f) for f in files)
 
@@ -75,7 +80,7 @@ def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
     newest = _deps_mtime()
     if not force and all(os.path.exists(p) and os.path.getmtime(p) >= newest
-                         for p in (LIB, DRAW_LIB, CONTOUR_LIB, COLOR_LIB, CORNERS_LIB, GROUP_LIB)):
+                         for p in (LIB, DRAW_LIB, CONTOUR_LIB, COLOR_LIB, CORNERS_LIB, GROUP_LIB, HOMOGRAPHY_LIB)):
         if not os.path.exists(os.path.join(HERE, "gsb_magick")):
             build_cli()
         return LIB
@@ -98,7 +103,8 @@ def build(force=False, verbose=False):
     color_srcs = [os.path.join(COLOR_DIR, f) for f in COLOR_SOURCES]
     corners_srcs = [os.path.join(CORNERS_DIR, f) for f in CORNERS_SOURCES]
     group_srcs = [os.path.join(GROUP_DIR, f) for f in GROUP_SOURCES]
-    companion_srcs = draw_srcs + contour_srcs + color_srcs + corners_srcs + group_srcs
+    homography_srcs = [os.path.join(HOMOGRAPHY_DIR, f) for f in HOMOGRAPHY_SOURCES]
+    companion_srcs = draw_srcs + contour_srcs + color_srcs + corners_srcs + group_srcs + homography_srcs
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES) + len(companion_srcs))) as ex:
         all_objs = list(ex.map(compile_one, SOURCES + companion_srcs))
     objs = all_objs[:len(SOURCES)]
@@ -107,8 +113,9 @@ def build(force=False, verbose=False):
     color_objs = all_objs[len(SOURCES) + len(draw_srcs) + len(contour_srcs):
                           len(SOURCES) + len(draw_srcs) + len(contour_srcs) + len(color_srcs)]
     corners_objs = all_objs[len(SOURCES) + len(draw_srcs) + len(contour_srcs) + len(color_srcs):
-                            len(all_objs) - len(group_srcs)]
-    group_objs = all_objs[len(all_objs) - len(group_srcs):]
+                            len(all_objs) - len(group_srcs) - len(homography_srcs)]
+    group_objs = all_objs[len(all_objs) - len(group_srcs) - len(homography_srcs):len(all_objs) - len(homography_srcs)]
+    homography_objs = all_objs[len(all_objs) - len(homography_srcs):]
     # export only the C ABI (gs_*); C++ symbols stay local
     vs = os.path.join(OBJ, "exports.map")
     with open(vs, "w") as f:
@@ -119,7 +126,7 @@ def build(force=False, verbose=False):
         raise RuntimeError("link failed:\n" + r.stdout + r.stderr)
     # the companions: each its own static cudart, the same export rule
     for lib, lib_objs in ((DRAW_LIB, draw_objs), (CONTOUR_LIB, contour_objs), (COLOR_LIB, color_objs),
-                         (CORNERS_LIB, corners_objs), (GROUP_LIB, group_objs)):
+                         (CORNERS_LIB, corners_objs), (GROUP_LIB, group_objs), (HOMOGRAPHY_LIB, homography_objs)):
         r = subprocess.run([cc, "-shared", "-o", lib] + lib_objs + ["-Xlinker", "--version-script=" + vs],
                            capture_output=True, text=True)
         if r.returncode != 0:
@@ -154,7 +161,7 @@ def write_cascade_header():
 
 
 def build_cli():
-    """gsb_magick: the C99 batch-pipeline CLI on the device-resident ABI (cli/gsb_magick.c), on all six libraries"""
+    """gsb_magick: the C99 batch-pipeline CLI on the device-resident ABI (cli/gsb_magick.c), on all seven libraries"""
     exe = os.path.join(HERE, "gsb_magick")
     write_cascade_header()
     cmd = ["gcc", "-std=c99", "-O2", "-Wall", "-Wextra", "-Werror", "-pedantic", "-D_POSIX_C_SOURCE=200809L",
@@ -162,7 +169,7 @@ def build_cli():
            os.path.join(HERE, "cli", "gsb_magick.c"),
            "-L" + HERE, "-l:" + os.path.basename(DRAW_LIB), "-l:" + os.path.basename(CONTOUR_LIB),
            "-l:" + os.path.basename(COLOR_LIB), "-l:" + os.path.basename(CORNERS_LIB),
-           "-l:" + os.path.basename(GROUP_LIB),
+           "-l:" + os.path.basename(GROUP_LIB), "-l:" + os.path.basename(HOMOGRAPHY_LIB),
            "-l:" + os.path.basename(LIB), "-Wl,-rpath,$ORIGIN"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

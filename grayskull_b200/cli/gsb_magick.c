@@ -4,7 +4,8 @@
  * libgrayskull_b200.so and, for the draw-* and faces stages, libgrayskull_draw.so (include/grayskull_draw.h), for
  * the contour stage libgrayskull_contour.so (include/grayskull_contour.h), for the contour and scan stages
  * libgrayskull_corners.so (include/grayskull_corners.h), for the faces-grouped stage libgrayskull_group.so
- * (include/grayskull_group.h), and for colour inputs libgrayskull_color.so (include/grayskull_color.h).
+ * (include/grayskull_group.h), for the find stage libgrayskull_homography.so (include/grayskull_homography.h), and for
+ * colour inputs libgrayskull_color.so (include/grayskull_color.h).
  *
  *   gsb_magick <pipeline> <out-prefix> in0.pgm|in0.ppm [in1 ...]
  *
@@ -48,6 +49,13 @@
  *   draw-orb:TEMPLATE.pgm (all the orb stage does, printed line included, then the verb's picture, nanomagick.c:313-343:
  *                    (tw + w) x max(th, h), template and frame side by side, lines for the 15 best matches.  Like the
  *                    verb, a frame without matches gets no output file; gsb_magick says so on stderr)
+ *   find:TEMPLATE.pgm:W:H (where the template lies in each frame: all the orb stage does, printed line included, then
+ *                    gs_b200_find_homography_batch with 1024 hypotheses, seed 0 and a 3 px threshold, and
+ *                    gs_b200_homography_quads_batch with at least 10 inliers -- choices of this tool, not reference
+ *                    values --; prints "frame F: found, I inliers, quad x0 y0 x1 y1 x2 y2 x3 y3" or "frame F: not
+ *                    found, I inliers", and warps each found quad to W x H with gs_b200_perspective_correct_batch, the
+ *                    scan stage's bilinear quad warp.  A frame not found gets no output file.  W and H are the last two
+ *                    fields, so the template path may hold ':')
  * e.g. the reference Makefile's lena chain:  blur:2,threshold:otsu,erode:2,dilate:2
  * Stage semantics are the reference's gs_* functions (same kernels as the drop-in gs_* entry points).
  */
@@ -60,6 +68,7 @@
 #include "grayskull_corners.h"
 #include "grayskull_draw.h"
 #include "grayskull_group.h"
+#include "grayskull_homography.h"
 #include "frontalface_cascade.h" /* generated by build.py from grayskull_b200/data/frontalface.npz */
 
 #define DIE(...) (fprintf(stderr, "gsb_magick: " __VA_ARGS__), fprintf(stderr, "\n"), exit(1))
@@ -83,13 +92,27 @@
   do {                                                                         \
     if ((call) != 0) DIE("%s failed: %s", #call, gs_b200_group_last_error());  \
   } while (0)
+#define CKH(call)                                                                   \
+  do {                                                                              \
+    if ((call) != 0) DIE("%s failed: %s", #call, gs_b200_homography_last_error());  \
+  } while (0)
 #define CKD(call)                                                             \
   do {                                                                        \
     if ((call) != 0) DIE("%s failed: %s", #call, gs_b200_draw_last_error());  \
   } while (0)
 
-/* frames that get no output file: the draw-orb stage's frames without matches, for which the verb writes no picture */
+/* frames that get no output file, and why: NO_MATCHES for the draw-orb stage's frames without matches, for which the
+ * verb writes no picture; NOT_FOUND for the find stage's frames where the template was not found */
+enum { NO_MATCHES = 1, NOT_FOUND = 2 };
 static unsigned char *g_no_output;
+
+static void no_output(unsigned f, unsigned n, unsigned char why) {
+  if (!g_no_output) {
+    g_no_output = (unsigned char *)calloc(n, 1);
+    if (!g_no_output) DIE("allocation failed");
+  }
+  g_no_output[f] = why;
+}
 
 struct batch {
   uint8_t *dev;
@@ -123,15 +146,16 @@ static size_t pyr_bytes(unsigned w, unsigned h, unsigned L, size_t *maps, size_t
   return pyr;
 }
 
-/* what the orb stage leaves on the device for draw-orb: the template, its one keypoint list, frame f's keypoints and
- * matches at stride ORB_NK / ORB_MM, and the match counts (also on the host, hm) */
+/* what the orb stage leaves on the device for draw-orb and find: the template, its one keypoint list tk and its copy
+ * per frame tks with the counts n1, frame f's keypoints, their counts scount and matches at stride ORB_NK / ORB_MM,
+ * and the match counts (also on the host, hm) */
 enum { ORB_NK = 2500, ORB_MM = 300 };
 struct orb_out {
   struct gs_image tpl;
   uint8_t *tdev;
-  struct gs_keypoint *tk, *sk;
+  struct gs_keypoint *tk, *tks, *sk;
   struct gs_match *matches;
-  unsigned *mcount, *hm;
+  unsigned *n1, *scount, *mcount, *hm;
 };
 
 /* the orb stage (see the header comment): template as set 1 of every pair, frame f's keypoints as set 2 */
@@ -205,14 +229,16 @@ static void orb_run(const char *path, const struct batch *cur, struct orb_out *o
   CK(gs_b200_memcpy_d2h(hm, mcount, sizeof(unsigned) * n, NULL));
   CK(gs_b200_stream_sync(NULL));
   for (f = 0; f < n; f++) printf("frame %u: Template: %u keypoints, Scene: %u keypoints, Matches: %u\n", f, ht, hs[f], hm[f]);
-  gs_b200_free(tbuf), gs_b200_free(tks), gs_b200_free(tcount);
+  gs_b200_free(tbuf), gs_b200_free(tcount);
   if (spyrd) gs_b200_free(spyrd);
-  gs_b200_free(ssm), gs_b200_free(scount), gs_b200_free(n1), free(htk), free(hs), free(h1);
-  o->tpl = tpl, o->tdev = tdev, o->tk = tk, o->sk = sk, o->matches = matches, o->mcount = mcount, o->hm = hm;
+  gs_b200_free(ssm), free(htk), free(hs), free(h1);
+  o->tpl = tpl, o->tdev = tdev, o->tk = tk, o->tks = tks, o->sk = sk, o->matches = matches, o->n1 = n1;
+  o->scount = scount, o->mcount = mcount, o->hm = hm;
 }
 
 static void orb_free(struct orb_out *o) {
-  gs_b200_free(o->tdev), gs_b200_free(o->tk), gs_b200_free(o->sk), gs_b200_free(o->matches), gs_b200_free(o->mcount);
+  gs_b200_free(o->tdev), gs_b200_free(o->tk), gs_b200_free(o->tks), gs_b200_free(o->sk), gs_b200_free(o->matches);
+  gs_b200_free(o->n1), gs_b200_free(o->scount), gs_b200_free(o->mcount);
   free(o->hm);
   gs_free(o->tpl);
 }
@@ -227,12 +253,59 @@ static void draw_orb_stage(const char *path, const struct batch *cur, struct bat
   CKD(gs_b200_draw_matches_batch(tmp->dev, cur->dev, cur->w, cur->h, cur->n, o.tdev, o.tpl.w, o.tpl.h, o.tk, 0, o.sk,
                                  ORB_NK, o.matches, o.mcount, ORB_MM, 15, NULL));
   CK(gs_b200_stream_sync(NULL));
-  if (!g_no_output) {
-    g_no_output = (unsigned char *)calloc(cur->n, 1);
-    if (!g_no_output) DIE("allocation failed");
-  }
   for (f = 0; f < cur->n; f++)
-    if (o.hm[f] == 0) g_no_output[f] = 1;
+    if (o.hm[f] == 0) no_output(f, cur->n, NO_MATCHES);
+  orb_free(&o);
+}
+
+/* find:TEMPLATE.pgm:W:H (see the header comment): the orb stage, then homography -> quad -> warp to W x H in *tmp */
+static void find_stage(const char *arg, const struct batch *cur, struct batch *tmp, size_t *cap_tmp) {
+  enum { HYP = 1024, MIN_INLIERS = 10 };
+  const char *c2 = strrchr(arg, ':'), *c1 = c2;
+  char path[4096];
+  unsigned f, n = cur->n, *inl, *hin;
+  int dw, dh;
+  double *H;
+  struct gs_point *corners, *hc;
+  uint8_t *found, *hf;
+  struct orb_out o;
+  while (c1 && c1 > arg && *--c1 != ':') {}
+  if (!c2 || !c1 || *c1 != ':' || c1 == arg || (size_t)(c1 - arg) >= sizeof(path))
+    DIE("bad find stage 'find:%s' (find:TEMPLATE.pgm:W:H)", arg);
+  dw = atoi(c1 + 1), dh = atoi(c2 + 1);
+  if (dw <= 0 || dh <= 0) DIE("bad size in 'find:%s'", arg);
+  memcpy(path, arg, (size_t)(c1 - arg));
+  path[c1 - arg] = 0;
+  orb_run(path, cur, &o);
+  H = (double *)gs_b200_malloc(sizeof(double) * 9 * n);
+  inl = (unsigned *)gs_b200_malloc(sizeof(unsigned) * n);
+  corners = (struct gs_point *)gs_b200_malloc(sizeof(*corners) * 4 * n);
+  found = (uint8_t *)gs_b200_malloc(n);
+  hin = (unsigned *)malloc(sizeof(unsigned) * n);
+  hc = (struct gs_point *)malloc(sizeof(*hc) * 4 * n);
+  hf = (uint8_t *)malloc(n);
+  if (!H || !inl || !corners || !found || !hin || !hc || !hf) DIE("allocation failed");
+  CKH(gs_b200_find_homography_batch(o.tks, o.n1, ORB_NK, o.sk, o.scount, ORB_NK, o.matches, o.mcount, ORB_MM, n, HYP,
+                                    0, 3.0, H, inl, NULL, NULL));
+  CKH(gs_b200_homography_quads_batch(H, inl, n, MIN_INLIERS, o.tpl.w, o.tpl.h, cur->w, cur->h, corners, found, NULL));
+  ensure(tmp, (unsigned)dw, (unsigned)dh, n, cap_tmp);
+  CK(gs_b200_perspective_correct_batch(tmp->dev, (unsigned)dw, (unsigned)dh, cur->dev, cur->w, cur->h, n, corners, 1,
+                                       NULL));
+  CK(gs_b200_memcpy_d2h(hin, inl, sizeof(unsigned) * n, NULL));
+  CK(gs_b200_memcpy_d2h(hc, corners, sizeof(*hc) * 4 * n, NULL));
+  CK(gs_b200_memcpy_d2h(hf, found, n, NULL));
+  CK(gs_b200_stream_sync(NULL));
+  for (f = 0; f < n; f++) {
+    const struct gs_point *q = hc + 4 * (size_t)f;
+    if (!hf[f]) {
+      printf("frame %u: not found, %u inliers\n", f, hin[f]);
+      no_output(f, n, NOT_FOUND);
+      continue;
+    }
+    printf("frame %u: found, %u inliers, quad %u %u %u %u %u %u %u %u\n", f, hin[f], q[0].x, q[0].y, q[1].x, q[1].y,
+           q[2].x, q[2].y, q[3].x, q[3].y);
+  }
+  gs_b200_free(H), gs_b200_free(inl), gs_b200_free(corners), gs_b200_free(found), free(hin), free(hc), free(hf);
   orb_free(&o);
 }
 
@@ -306,6 +379,8 @@ static void stage(const char *spec, struct batch *cur, struct batch *tmp, size_t
     orb_free(&o);
   } else if (!strncmp(spec, "draw-orb:", 9) && spec[9]) {
     draw_orb_stage(spec + 9, cur, tmp, cap_tmp);
+  } else if (!strncmp(spec, "find:", 5) && spec[5]) {
+    find_stage(spec + 5, cur, tmp, cap_tmp);
   } else if (!strcmp(name, "draw-keypoints") && nargs == 2) {
     /* nanomagick.c:217-242: gs_fast into a zeroed score map with cap 5000, then the crosses of the N strongest */
     enum { CAP = 5000 };
@@ -608,7 +683,8 @@ int main(int argc, char **argv) {
       img.w = cur.w, img.h = cur.h, img.data = hout + frame_bytes(&cur) * f;
       snprintf(path, sizeof(path), "%s%04u.pgm", argv[2], f);
       if (g_no_output && g_no_output[f]) {
-        fprintf(stderr, "gsb_magick: frame %u: no matches, %s not written\n", f, path);
+        fprintf(stderr, "gsb_magick: frame %u: %s, %s not written\n", f,
+                g_no_output[f] == NO_MATCHES ? "no matches" : "template not found", path);
         continue;
       }
       if (gs_write_pgm(img, path) != 0) DIE("could not write %s", path);
